@@ -3,6 +3,7 @@
 G+D train step (batch 300 per GPU, synthetic clean/noisy pairs, RMSprop, LSGAN + L1).
 
     python bench.py --gpus 1 --steps 20 --warmup 5
+    python bench.py --gpus 1 --steps 20 --warmup 5 --dump-outputs DIR   # + what the last timed step computed
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
     python bench.py --impl reference ...        # the reference's CPU path (oracle port), host cores
 
@@ -11,7 +12,7 @@ D(fake) fwd + dgrad through the updated D, L1, G bwd, G RMSprop (segan/models/mo
 `value`  : device-timed (CUDA events), inputs already resident in HBM.
 `e2e`    : same step through SEGAN.train's per-batch path with pinned HOST buffers: H2D copy of the
            batch and D2H read of the four losses inside the timed region.
-`roofline`: the dominant kernel (tcgen05 forward-form tap-GEMM), algorithmic FLOPs / CUDA-event time.
+`roofline`: the dominant kernel (wgmma forward-form tap-GEMM), algorithmic FLOPs / CUDA-event time.
 `cpu_baseline`: the oracle (CPU restatement of the reference step) on this box's host cores.
 """
 import argparse
@@ -21,6 +22,7 @@ import subprocess
 import sys
 import threading
 import time
+import zlib
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 if ROOT not in sys.path:
@@ -40,18 +42,19 @@ def measured_peaks():
             d = json.load(f)
         return dict(tflops=float(d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1590.0))),
                     hbm=float(d.get("hbm_gbs", 6650.0)), src="measured (MEASURED_PEAKS.json, sustained)")
-    return dict(tflops=1400.0, hbm=6650.0, src="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W): dense FP16 tensor rate, HBM3 bandwidth -- not reached figures
+    return dict(tflops=989.0, hbm=3350.0, src="H100 SXM data sheet (dense FP16, 700 W)")
 
 
-def ncu_traffic():
+def ncu_traffic(path=None):
     """DRAM bytes per launch of the dominant kernel (dram__bytes_read.sum + dram__bytes_write.sum, average over the
-    launches of one train step) from the committed step-level ncu capture of this round
-    (profiles/r2_step_traffic.json <- tools/step_traffic.py + tools/ncu_step_summary.py), or None when it is missing."""
-    p = os.path.join(ROOT, "profiles", "r2_step_traffic.json")
+    launches of one train step) from a step-level ncu capture summarised by tools/ncu_step_summary.py (default:
+    profiles/step_traffic.json, see tools/step_traffic.py), or None when there is none."""
+    p = path or os.path.join(ROOT, "profiles", "step_traffic.json")
     try:
         with open(p) as f:
             ks = json.load(f)["kernels"]
-        hits = [v for k, v in ks.items() if k.startswith("tapgemm_f_tc2")]
+        hits = [v for k, v in ks.items() if k.startswith("tapgemm_f_tc")]
         n = sum(v["launches"] for v in hits)
         return sum(v["dram_read_bytes"] + v["dram_write_bytes"] for v in hits) / n if n else None
     except Exception:
@@ -59,7 +62,7 @@ def ncu_traffic():
 
 
 class ClockSampler(object):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -105,6 +108,29 @@ class ClockSampler(object):
         sm.sort()
         return dict(sm_mhz=(sm[len(sm) // 2] if sm else None), sm_max_mhz=smax, reasons=sorted(reasons),
                     samples=len(sm))
+
+
+DUMP_SAMPLE = 4096     # entries kept per state tensor by --dump-outputs (fixed, seeded positions)
+
+
+def dump_outputs(out_dir, s, losses):
+    """What the timed path hands its caller after its last step: the step's four losses and the updated G / D
+    state (reference-layout state_dict, as a checkpoint would hold it), the latter as a fixed, seeded sample of
+    DUMP_SAMPLE entries per tensor, concatenated in state_dict order."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "losses.npy"), losses.detach().float().cpu().numpy())
+    for name, mod in (("G", s.G), ("D", s.D)):
+        parts = []
+        for k, v in mod.state_dict().items():
+            if not v.dtype.is_floating_point:
+                continue
+            flat = v.detach().float().reshape(-1).cpu().numpy()
+            if flat.size > DUMP_SAMPLE:
+                rs = np.random.RandomState(zlib.crc32(k.encode()))
+                flat = flat[np.sort(rs.choice(flat.size, DUMP_SAMPLE, replace=False))]
+            parts.append(flat)
+        np.save(os.path.join(out_dir, "%s_state_sample.npy" % name), np.concatenate(parts).astype(np.float32))
 
 
 def synth_batch(B, seed):
@@ -365,7 +391,7 @@ def gpu_extras(dev, B, s_plus):
 # our arm
 # ----------------------------------------------------------------------------------------------
 def _claim_stdout():
-    """The driver reads ONE JSON line from stdout: native libraries (NCCL prints its version banner
+    """A caller reads ONE JSON line from stdout: native libraries (NCCL prints its version banner
     there) are pointed at stderr for the whole run; the returned writer emits on the real stdout."""
     sys.stdout.flush()
     real = os.dup(1)
@@ -386,7 +412,7 @@ def _guard(fn, *a):
 
 def _leave(world):
     """End of a data-parallel run: the step's CUDA graph holds captured NCCL kernels, and tearing the process group
-    down under it was seen to block (2 x B200: the JSON line was out, destroy_process_group() never returned).  Every
+    down under it was seen to block (2 GPUs: the JSON line was out, destroy_process_group() never returned).  Every
     rank has passed its last collective when it gets here, all device work is drained, so the process simply ends."""
     if world > 1:
         import torch.distributed as dist
@@ -411,7 +437,9 @@ def main():
     ap.add_argument("--cpu-baseline-steps", type=int, default=3)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip BASELINE configs 4 / 5 (extra keys)")
-    ap.add_argument("--backend", default=None, help="tcgen05 (default) | ffma")
+    ap.add_argument("--backend", default=None, help="tcgen05 (default: the wgmma tensor-core kernels) | ffma")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed as DIR/<name>.npy")
     args = ap.parse_args()
     if args.warmup < 3 and args.impl == "b200":
         args.warmup = 3
@@ -428,14 +456,14 @@ def main():
     dev = torch.device("cuda", local_rank)
     if world > 1:
         # NCCL_DEBUG is left as the launcher set it: fd 1 already points at stderr (_claim_stdout), so NCCL's INFO
-        # lines (communicator / rank evidence the driver greps for) cannot pollute the one JSON line
+        # lines (communicator / rank evidence) cannot pollute the one JSON line
         dist.init_process_group("nccl", device_id=dev)
     from segan_pytorch_b200 import _lib, engine as E
     from segan_pytorch_b200.hostbind import bind_host_to_gpu
     from tests.util import build_segan, load_opts
     numa_cpus = bind_host_to_gpu(dev)          # before any pinned staging buffer is allocated
     if not _lib.device_ok():
-        raise SystemExit("bench.py needs an sm_100-class GPU and libsegan_b200.so (no fallback path)")
+        raise SystemExit("bench.py needs an H100 (sm_90) GPU and libsegan_b200.so (no fallback path)")
     B = args.batch
     opts = load_opts(batch_size=B, z_device="cuda")
     s = build_segan(seed=111, batch_size=B, z_device="cuda").to(dev)      # identical init on every rank
@@ -486,6 +514,8 @@ def main():
     barrier()
     ms = e0.elapsed_time(e1)
     mark("timed region done: %.3f ms/step" % (ms / args.steps))
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, s, losses)
     launches = _lib.launch_count - launches0
     ngraphs = [len(v.graphs) for v in getattr(s, "_step_graphs", {}).values() if getattr(v, "graphs", None) is not None]
     clocks = sampler.stop() if rank == 0 else None
@@ -644,7 +674,7 @@ def main():
         alg_fl = ALG_GFLOP_F_PER_WINDOW * 1e9 * B * args.steps if dom == "tapgemm_f" else fl
         alg_fl = min(alg_fl, fl)
         ach = alg_fl / sec / 1e12
-        roof = {"kernel": dom + "_tc2 (tcgen05 cta_group::2 tap-GEMM)", "bound": "tensor", "achieved": ach,
+        roof = {"kernel": dom + "_tc (wgmma tap-GEMM)", "bound": "tensor", "achieved": ach,
                 "peak": peaks["tflops"], "unit": "TFLOP/s", "frac": ach / peaks["tflops"], "traffic": ncu_traffic(),
                 "peak_source": peaks["src"], "avg_launch_ms": sec * 1e3 / n,
                 "alg_flops_per_launch": alg_fl / n, "executed_flops_per_launch": fl / n,
@@ -673,7 +703,7 @@ def main():
                                     "/".join(str(n) for n in ngraphs) or "?",
                                     " (NCCL all-reduce chunks captured inside)" if world > 1 and ngraphs == [1] else "")
                                  if graphs_on else ", eager launches")),
-                   "l2": "per-step working set (packed weights 0.4 GB + activations > 2 GB) exceeds the 126 MB L2"},
+                   "l2": "per-step working set (packed weights 0.4 GB + activations > 2 GB) exceeds the 50 MB L2"},
         "clocks": clocks,
         "e2e": {"value": e2e_value, "unit": "windows/s", "ms_per_step": ms_e2e / args.steps,
                 "h2d_bytes_per_step": h2d_per_step, "d2h_bytes_per_step": 16, "last_losses": host_loss,

@@ -1,9 +1,9 @@
 /*
- * segan_b200.h -- C ABI of libsegan_b200.so: the B200 (sm_100a) kernels underneath the
+ * segan_b200.h -- C ABI of libsegan_b200.so: the H100 (sm_90a) kernels underneath the
  * santi-pdp/segan_pytorch Python API (Generator / Discriminator / SEGAN train step).
  *
  * The reference has no FFI of its own (it is pure Python over torch ops; SURVEY.md 8b): every
- * entry point below names the reference call site (file:line under /root/reference) whose
+ * entry point below names the reference call site (file:line in santi-pdp/segan_pytorch) whose
  * library dispatch it replaces.  Conventions:
  *   - plain pointers + sizes, no torch types; every pointer is a DEVICE pointer unless noted
  *   - the caller owns all memory (outputs and workspaces included); nothing is retained
@@ -58,15 +58,14 @@ extern "C" {
 
 /* tap-GEMM back ends */
 #define SG_BACKEND_FFMA 0    /* CUDA-core fp32 reference implementation (validation / fallback) */
-#define SG_BACKEND_TCGEN05 1 /* TMA + tcgen05.mma + TMEM (the product path) */
+#define SG_BACKEND_TCGEN05 1 /* TMA + mbarrier + wgmma tensor cores (the product path; name kept for the ABI) */
 
 int sg_abi_version(void);
 const char* sg_last_error(void);
-/* 1 if the loaded device is sm_100 class and the tcgen05 kernels can run */
+/* 1 if the current device is compute capability 9.0 (H100) and the sm_90a kernels can run */
 int sg_device_ok(void);
-/* Forward-form tap-GEMM kernel: 0 = single-CTA 128-row tiles; 1 = CTA pairs (tcgen05 cta_group::2, 256-row
- * tiles); 2 = CTA pairs with the activation tile staged once per k-block and reused by all taps through
- * row-shifted UMMA descriptors (layers with >= 128 rows per batch element; others fall back to 1).
+/* Forward-form tap-GEMM schedule selector (0 | 1 | 2), kept for ABI compatibility: the sm_90a library has one
+ * forward-form kernel (128-row tiles, two consumer warpgroups) and runs it for every setting.
  * Returns the previous setting.  Environment default: SEGAN_B200_CTA_PAIR. */
 int sg_set_cta_pair(int on);
 /* Tuning knobs of the HBM-bound streaming kernels, one per kernel family (`kind`):
@@ -89,15 +88,15 @@ int sg_set_ew_variant(int kind, int vec, int unroll, int cap);
 /* 16-bit format of every GRADIENT tensor the library reads or writes (the `g_*` arguments below, the col2im input,
  * the D head's g_z1): SG_F16 (default) or SG_BF16.  Returns the previous setting.
  * fp16 gradients carry 11 significant bits (bf16: 8) and share the forward tensors' format, so the weight-gradient
- * tap-GEMM reads the forward activations directly (tcgen05 kind::f16 cannot mix f16 x bf16 operands: with bf16
+ * tap-GEMM reads the forward activations directly (wgmma cannot mix f16 x bf16 operands: with bf16
  * gradients every forward activation needs a bf16 twin).  Their narrower range is covered by a loss scale: the
  * `grad_scale` argument of sg_fc_tail_bwd / sg_l1_loss_bwd multiplies the loss gradients at their source, every
  * parameter gradient then carries the factor and the optimiser's `grad_scale` divides it out; 16-bit stores
  * saturate at +-65504.  (autograd in model.py:299,306,320 keeps fp32 gradients: this is the precision contract
  * of north_star's "fp16/bf16 sample windows".) */
 int sg_set_grad_dtype(int dtype);
-/* Split-K over the last, partial wave of sg_tapgemm_f_run's CTA-pair kernel (needs sg_tapgemm_f.sk_ws):
- * max_split = largest number of CTA pairs one leftover tile is split over (0 | 1 = off, default 16; < 0 keeps it);
+/* Split-K over the last, partial wave of sg_tapgemm_f_run's tensor-core kernel (needs sg_tapgemm_f.sk_ws):
+ * max_split = largest number of CTAs one leftover tile is split over (0 | 1 = off, default 16; < 0 keeps it);
  * atomic_steps = cost-model constant: the finisher's cost of adding one 256-wide partial tile, in k-steps (<= 0
  * keeps it; a value below 1e-3 also drops the model's fixed cost, i.e. forces the split -- sweeps and tests).
  * Returns the previous max_split.  Environment: SEGAN_B200_STREAMK, SEGAN_B200_SK_ATOMIC. */
@@ -138,33 +137,33 @@ typedef struct sg_tapgemm_f {
   int32_t batch;
   int32_t ksplit;     /* >1 only with out_dtype == SG_F32 */
   int32_t backend;    /* SG_BACKEND_* */
-  int32_t tile_n;     /* N tile of the tcgen05 kernel: 0 = widest of 256/128/64 dividing n_hi-n_lo; 64|128|256 =
-                         narrower tiles for the tail of a launch split against wave quantisation (148 SMs) */
+  int32_t tile_n;     /* N tile of the tensor-core kernel: 0 = widest of 256/128/64 dividing n_hi-n_lo; 64|128|256 =
+                         narrower tiles for the tail of a launch split against wave quantisation (132 SMs) */
   double* bn_stats;   /* or NULL.  Fused nn.BatchNorm1d batch statistics (modules.py:11,100) of the output: per
                          column sum and sum of squares of the stored (rounded) values over all computed rows,
                          accumulated into [SG_STAT_SLICES][2][nc] doubles (same buffer sg_bn_stats fills; caller
-                         zeroes).  tcgen05 backend, 16-bit out, ksplit 1, n_lo = 0, n_hi = nc, >= 2 M tiles. */
+                         zeroes).  Tensor-core backend, 16-bit out, ksplit 1, n_lo = 0, n_hi = nc. */
   void* out2;         /* or NULL.  Fused second output out2[b][out2_halo + m][n] = PReLU_slope[n % slope_mod](out value), same
                          dtype / row pitch / column mapping as `out`, own halo: the consumer-ready activation of a Generator
                          block whose contraction feeds PReLU directly (modules.py:99-101,139-141; no norm layer), stored
                          next to the raw pre-activation the skip connection needs (generator.py:185,191).  With
                          out2_halo > 0 (reflect padding of the next conv, modules.py:92-98) position m is also written to
                          its mirror row -m or 2(out_rows-1)-m when it lies within out2_halo of an end; needs m_lo = 0,
-                         m_hi = out_rows, out_rows >= 2*out2_halo + 3.  tcgen05 backend, CTA-pair kernel, 16-bit out. */
+                         m_hi = out_rows, out_rows >= 2*out2_halo + 3.  Tensor-core backend, 16-bit out. */
   int32_t out2_halo;
   const float* slope; /* with out2 == NULL and slope != NULL the PReLU is applied to `out` itself (inference decoder) */
   int32_t slope_mod;
   void* sk_ws;        /* or NULL.  Zero-initialised workspace of sg_tapgemm_f_workspace_bytes() bytes that lets the
-                         CTA-pair kernel split the tiles of its last, partial wave along K over several CTA pairs (fp32
-                         partial sums in per-pair slots, summed in slot order by whoever finishes a tile: deterministic;
+                         tensor-core kernel split the tiles of its last, partial wave along K over several CTAs (fp32
+                         partial sums in per-CTA slots, summed in slot order by whoever finishes a tile: deterministic;
                          counters, which the kernel leaves zeroed).  One workspace per stream: launches that may run
-                         concurrently must not share it.  (bias / slope must be 16-byte aligned for that kernel.) */
+                         concurrently must not share it. */
 } sg_tapgemm_f;
 
 int sg_tapgemm_f_run(const sg_tapgemm_f* p, void* stream);
 /* size of sg_tapgemm_f.sk_ws (device memory, zero-filled once by the caller) */
 int64_t sg_tapgemm_f_workspace_bytes(void);
-/* Diagnostics (SEGAN_B200_DEBUG bit 20): per-CTA phase timeline of the last CTA-pair tap-GEMM launch, 32 globaltimer
+/* Diagnostics (SEGAN_B200_DEBUG bit 20): per-CTA phase timeline of the last forward-form tap-GEMM launch, 32 globaltimer
  * words (ns) per CTA for up to 160 CTAs -- [0] start, then per tile piece: accumulator ready, epilogue done, (split
  * tiles, bit 63 set) finisher done; last non-zero word = exit.  Copies min(max_words, 5120) words to the HOST buffer
  * and returns the count (-1 on a CUDA error).  Not used by the product path. */
@@ -274,7 +273,7 @@ int sg_bn_finalize(const double* stats, int64_t count, int C, const float* gamma
  * reflect halo (the consumer's view).  scale_shift may be NULL.  a: [B][L][C] exact.
  * out_halo_pos = halo in positions (0 or 16).  act: SG_ACT_NONE|SG_ACT_PRELU.
  * The bf16 twins feed the weight-gradient tap-GEMM, whose two operands must share one 16-bit
- * format (tcgen05 kind::f16 rejects f16 x bf16; gradients are bf16 for range). */
+ * format (wgmma rejects f16 x bf16; gradients are bf16 for range). */
 int sg_act_fwd(const void* a, int dtype, int batch, int L, int C, const float* scale_shift,
                const float* slope, int act, int roll, const int32_t* roll_dev, int out_halo_pos, void* h,
                void* h_bf16 /* optional bf16 twin of h (same geometry) */,

@@ -1,9 +1,8 @@
 """TEST INFRASTRUCTURE ONLY -- loader for the *unmodified* reference (santi-pdp/segan_pytorch).
 
-Used only in the authoring container (where /root/reference exists) by
-tests/golden/make_golden.py and by the not-gpu test that pins the oracle restatement
-(oracle/segan_oracle.py) against the reference itself.  /root/reference does not exist on the
-GPU box, so nothing under `-m gpu`, smoke() or bench.py calls this.
+Used only by tests/golden/make_golden.py, which executes the reference to write the committed fixtures
+under tests/golden/; the location of a reference checkout comes from SEGAN_REFERENCE_ROOT.  Nothing in
+the test-suite, smoke() or bench.py calls this.
 
 Recipe = SURVEY.md App. D: six stub modules for un-installed, un-needed dependencies, oneDNN
 disabled (finding F1: the multi-threaded oneDNN fp32 conv_transpose1d forward is numerically
@@ -17,11 +16,11 @@ import os
 import sys
 import types
 
-REFERENCE_ROOT = os.environ.get("SEGAN_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("SEGAN_REFERENCE_ROOT", "")
 
 
 def reference_available():
-    return os.path.isdir(os.path.join(REFERENCE_ROOT, "segan", "models"))
+    return bool(REFERENCE_ROOT) and os.path.isdir(os.path.join(REFERENCE_ROOT, "segan", "models"))
 
 
 def _stub(name, **kw):
@@ -52,7 +51,7 @@ def load_reference():
     if _loaded is not None:
         return _loaded
     if not reference_available():
-        raise RuntimeError("reference tree not present at %s" % REFERENCE_ROOT)
+        raise RuntimeError("no reference checkout: set SEGAN_REFERENCE_ROOT (got %r)" % REFERENCE_ROOT)
     import torch
     torch.backends.mkldnn.enabled = False  # F1
     for n in ("librosa", "soundfile", "h5py", "ahoproc_tools", "ahoproc_tools.io",

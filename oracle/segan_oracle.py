@@ -10,7 +10,7 @@ Parity status: PINNED.  tests/test_oracle_pinned.py checks every function here a
 (b) the golden vectors that tests/golden/make_golden.py generated from that same reference
 (the reference itself ships no tests / golden vectors -- SURVEY.md section 4).
 
-All `file:line` citations are into /root/reference (commit 0522387).
+All `file:line` citations are into santi-pdp/segan_pytorch (commit 0522387).
 
 oneDNN is switched off for every call made here (SURVEY.md finding F1: the multi-threaded
 oneDNN fp32 conv_transpose1d forward is wrong for the dec_blocks.0-2 shapes in this image).
@@ -57,7 +57,7 @@ def onednn_as_configured():
 
 
 # --------------------------------------------------------------------------------------
-# operand-precision control (tests only).  The B200 path feeds its tensor cores 16-bit operands (fp16
+# operand-precision control (tests only).  The CUDA path feeds its tensor cores 16-bit operands (fp16
 # activations and weights, fp32 accumulation) and stores layer outputs in fp16.  Inside
 # `with operand_precision(torch.float16):` the three contraction primitives below round their inputs, weights
 # and outputs the same way while everything else stays the fp32 reference arithmetic: the distance between this

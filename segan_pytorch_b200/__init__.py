@@ -1,4 +1,4 @@
-"""segan_pytorch_b200 -- B200-native (sm_100a) engine for the SEGAN+ hot path of
+"""segan_pytorch_b200 -- H100-native (sm_90a) engine for the SEGAN+ hot path of
 santi-pdp/segan_pytorch: Generator / Discriminator conv stacks, the G+D LSGAN train step and
 G-only streaming inference, behind the reference's Python API (`segan_pytorch_b200.segan`,
 also importable as top-level `segan`).  Compute lives in libsegan_b200.so (C ABI:

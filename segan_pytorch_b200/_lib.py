@@ -1,6 +1,6 @@
 """ctypes binding of libsegan_b200.so (the C ABI declared in include/segan_b200.h).
 
-The library is the product: if it is missing, not loadable, or the device is not sm_100 class,
+The library is the product: if it is missing, not loadable, or the device is not an H100 (sm_90),
 every compute entry point raises -- there is no CPU / ATen fallback behind this module.
 """
 import ctypes as C

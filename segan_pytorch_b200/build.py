@@ -1,4 +1,4 @@
-"""Builds libsegan_b200.so in-tree with nvcc for sm_100a (no torch headers: the library is a
+"""Builds libsegan_b200.so in-tree with nvcc for sm_90a (H100) (no torch headers: the library is a
 plain C ABI).  `python -m segan_pytorch_b200.build` or __graft_entry__.build()."""
 import os
 import subprocess
@@ -8,7 +8,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libsegan_b200.so")
 SOURCES = ["api.cu", "tapgemm_ref.cu", "tapgemm_tc.cu", "wave_layers.cu", "elementwise.cu", "stream_ew.cu", "optim_pack.cu", "snorm.cu", "stft.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
@@ -46,7 +46,7 @@ def build(force=False, verbose=False):
     if failed:
         raise RuntimeError("nvcc failed building libsegan_b200.so")
     tmp = LIB + ".tmp.%d" % os.getpid()          # link aside, then rename: a reader never sees a half-written library
-    cmd = [_nvcc(), "-shared", "-o", tmp] + objs + ["-lcudart"]
+    cmd = [_nvcc(), "-shared"] + NVCC_FLAGS[:2] + ["-o", tmp] + objs + ["-lcudart"]
     subprocess.check_call(cmd)
     os.replace(tmp, LIB)
     return LIB

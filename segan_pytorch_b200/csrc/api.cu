@@ -53,9 +53,10 @@ extern "C" int sg_set_grad_dtype(int dtype) {
 extern "C" int sg_device_ok(void) {
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return 0;
-  int major = 0;
+  int major = 0, minor = 0;
   if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return 0;
-  return major == 10 ? 1 : 0;
+  if (cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev) != cudaSuccess) return 0;
+  return (major == 9 && minor == 0) ? 1 : 0;      // sm_90a code loads on compute capability 9.0 only
 }
 
 static int check_taps(const int32_t* k_lo, const int32_t* k_hi, const int32_t* n_lo, const int32_t* n_hi, int d_lo,
@@ -99,7 +100,7 @@ extern "C" int sg_tapgemm_f_run(const sg_tapgemm_f* p, void* stream) {
   }
   if (p->backend == SG_BACKEND_FFMA) {
     if (p->bn_stats != nullptr || p->out2 != nullptr || p->slope != nullptr) {
-      set_error("bn_stats / out2 (fused epilogues) need the tcgen05 backend");
+      set_error("bn_stats / out2 (fused epilogues) need the tensor-core backend");
       return SG_ERR_UNSUPPORTED;
     }
     return tapgemm_f_ffma_launch(p, (cudaStream_t)stream);
@@ -120,7 +121,7 @@ extern "C" int sg_tapgemm_w_run(const sg_tapgemm_w* p, void* stream) {
   SG_CHECK_ARG(p->a_dtype == SG_F16 || p->a_dtype == SG_BF16);
   SG_CHECK_ARG(p->batch > 0 && p->g_rows > 0 && (p->g_rows >= 64 ? p->g_rows % 64 == 0 : 64 % p->g_rows == 0));
   if (p->backend == SG_BACKEND_TCGEN05) {
-    // tcgen05.mma kind::f16 raises an illegal-instruction fault for f16 x bf16 (measured on B200)
+    // wgmma takes A and B in one 16-bit format
     SG_CHECK_ARG(p->g_dtype == p->a_dtype);
     return tapgemm_w_tc_launch(p, (cudaStream_t)stream);
   }

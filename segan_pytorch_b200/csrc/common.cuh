@@ -1,4 +1,4 @@
-// Shared helpers for libsegan_b200 (sm_100a only).
+// Shared helpers for libsegan_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -44,7 +44,7 @@ extern int g_grad_dtype;
 
 constexpr int KW = 31;      // kernel width (train.opts gkwidth)
 constexpr int NTAP = 9;     // row taps d in [-4, 4] of the stride-1 "row" formulation
-constexpr int NUM_SMS = 148;
+constexpr int NUM_SMS = 132;    // H100 SXM
 
 __host__ __device__ inline int64_t cdiv(int64_t a, int64_t b) { return (a + b - 1) / b; }
 

@@ -12,7 +12,7 @@ namespace sg {
 // ------------------------------------------------------------------------------------------
 // Streaming kernels.  Thread = VEC adjacent channels (one 8- or 16-byte load per stream) of a row,
 // C/VEC threads per row, 256/(C/VEC) rows per CTA iteration, UNROLL rows in flight per thread.
-// The per-thread bytes in flight (loads x VEC x 2 B x UNROLL) are what matters on B200: these
+// The per-thread bytes in flight (loads x VEC x 2 B x UNROLL) are what matters here: these
 // kernels also run CONCURRENTLY with the persistent tap-GEMMs (engine.py side streams), where only
 // 2-3 of their CTAs fit next to a GEMM CTA on an SM, so memory-level parallelism has to come from
 // the thread, not from occupancy.  The variant (VEC, UNROLL, grid caps) is a runtime tuning knob
@@ -219,7 +219,7 @@ act_fwd_kernel(const void* __restrict__ a, int dtype, int batch, int L, int C,
           if (act == SG_ACT_PRELU) y[j] = y[j] > 0.f ? y[j] : sl[j] * y[j];
         }
         stv<VEC>(h, (int64_t)r * C + cg * VEC, y, dtype);
-        // bf16 twins: operands of the weight-gradient tap-GEMM (tcgen05 kind::f16 cannot mix f16 x bf16)
+        // bf16 twins: operands of the weight-gradient tap-GEMM (wgmma cannot mix f16 x bf16 operands)
         if (h_bf16) stv<VEC>(h_bf16, (int64_t)r * C + cg * VEC, y, SG_BF16);
         if (a_bf16 && srcs[u] >= 0) stv<VEC>(a_bf16, (int64_t)srcs[u] * C + cg * VEC, v.v, SG_BF16);
       }
@@ -830,7 +830,7 @@ int launch_act_bwd_bulk(const void* g_h, int H, int roll, const int32_t* roll_de
                         const float* mean_invstd, const float* slope, int act, const double* red_in, double* red_out,
                         int use_bn, void* g_a_out, cudaStream_t st);
 
-// Defaults = the best of tools/ew_sweep.py on B200 (profiles/r2_ew_sweep.txt): the TMA-staged kernels (vec 16) wherever
+// Defaults (tools/ew_sweep.py compares the variants): the TMA-staged kernels (vec 16) wherever
 // they apply -- contiguous 16-bit tensors without twins -- else the register-staged (8, 4, 2); BatchNorm statistics
 // (one read-only stream) gain nothing from staging and stay register-staged.
 struct EwVariant { int vec, unroll, cap; };

@@ -2,9 +2,8 @@
 // with reflect halo + phase shift, and the two passes of their backward).
 //
 // The register-staged versions in elementwise.cu keep 32-48 KB of loads in flight per SM (256-thread CTAs x 2, a few
-// 16-byte loads per thread) and measure 2.2-3.9 TB/s on B200 where a device copy reaches 5.4 (tools/ew_sweep.py):
-// with ~1 us of loaded HBM latency, 6.5 TB/s needs > 50 KB in flight per SM and the register file cannot hold that
-// next to the per-channel accumulators.  Here the bytes in flight live in shared memory instead: one producer thread
+// 16-byte loads per thread).  With ~1 us of loaded HBM latency, streaming at HBM rate needs more bytes in flight per SM
+// than the register file can hold next to the per-channel accumulators.  Here the bytes in flight live in shared memory instead: one producer thread
 // per CTA streams contiguous row tiles with cp.async.bulk (1-D TMA, mbarrier complete_tx) through a ring of 16 KB
 // stages -- 64-96 KB in flight per CTA, two CTAs per SM -- and eight consumer warps read the tiles with
 // conflict-free 16-byte shared loads.  Outputs are coalesced 16-byte global stores.

@@ -1,6 +1,6 @@
 // CUDA-core (fp32 FFMA) implementation of the two tap-GEMM forms.  This is the validation /
 // fallback back end (SG_BACKEND_FFMA): same operands, same HBM layouts and same semantics as
-// the tcgen05 kernels in tapgemm_tc.cu, written the obvious way so that it can serve as an
+// the wgmma kernels in tapgemm_tc.cu, written the obvious way so that it can serve as an
 // on-device cross-check for them.  It is NOT the performance path.
 #include "common.cuh"
 

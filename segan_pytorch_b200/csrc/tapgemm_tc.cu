@@ -1,16 +1,16 @@
-// tcgen05 / TMA / TMEM implementation of the two tap-GEMM forms (SG_BACKEND_TCGEN05), sm_100a.
+// TMA / mbarrier / wgmma implementation of the two tap-GEMM forms (SG_BACKEND_TCGEN05), sm_90a.
 //
-// Both kernels are persistent (one CTA per SM, static round-robin tile schedule), warp
-// specialised -- warp 0: TMA producer, warp 1: TMEM allocator + single-thread tcgen05.mma
-// issuer, warps 2..5: epilogue (TMEM -> registers -> HBM) -- with a 4-stage smem ring
-// (full/empty mbarriers) and a double-buffered 128 x 256 fp32 accumulator in TMEM
-// (tmem_full/tmem_empty mbarriers) so that the epilogue of tile i overlaps the main loop of
-// tile i+1.
+// Both kernels are persistent (at most one CTA per SM, static round-robin tile schedule) and warp
+// specialised by warpgroup -- warpgroup 0: TMA producer (one thread issues, the others give their
+// registers back with setmaxnreg), warpgroups 1 and 2: consumers, each owning 64 of the tile's 128 M rows
+// with its fp32 accumulator in registers (wgmma m64nNk16, N = the tile's width) and storing its own rows
+// in the epilogue.  A 4-stage shared-memory ring (full / empty mbarriers) keeps the producer ahead of
+// the consumers, so the loads of tile i+1 overlap the epilogue of tile i.
 //
 // Every operand tile is a TMA box of 64 channels (128 B) x rows, 128B-swizzled, so the same
-// smem bytes serve as
-//   * a K-major  UMMA operand (rows = M/N, 64 channels = K)   -> form F (fwd / dgrad)
-//   * an MN-major UMMA operand (64 channels = M/N, rows = K)  -> form W (wgrad)
+// shared-memory bytes serve as
+//   * a K-major  wgmma operand (rows = M/N, 64 channels = K)   -> form F (fwd / dgrad)
+//   * an MN-major wgmma operand (64 channels = M/N, rows = K)  -> form W (wgrad)
 // i.e. no im2col, no transposed copies in HBM: the 9 row-taps are just 9 different TMA
 // coordinates into the same NLC-row tensor.
 #include "common.cuh"
@@ -81,121 +81,135 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, u
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols));
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
+// 8-byte vector reduction (sm_90+): one RED for two fp32 adds
+__device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols));
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+// the 256 consumer threads of a CTA (named barrier 1; the producer warpgroup never joins it)
+__device__ __forceinline__ void consumer_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
+// wgmma m64nNk16, fp32 accumulators in registers, both operands from shared memory through descriptors.
+// TA / TB: 0 = K-major operand, 1 = MN-major (transposed) operand.  scale_d = 0 starts a new accumulation.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_f16_n64(float (&d)[32], uint64_t da, uint64_t db, int scale_d) {
   asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrives (count 1) on `bar` once all previously issued tcgen05.mma of this thread retire
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-// 16-byte vector reduction (sm_90+): one RED for four fp32 adds
-__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// One lane of a fully converged warp.  The MMA warps run their loops warp-uniformly and only ISSUE through
-// the elected lane: descriptors, barrier addresses and counters computed in uniform control flow reach the
-// UTCHMMA / UTCBAR instructions through uniform registers.  With the whole loop under `if (lane == 0)` every
-// operand went through an ELECT + 5 x R2UR.BROADCAST + BRA.U.ANY "waterfall" (cuobjdump), ~90 cycles per
-// tcgen05.mma, and that single thread paced the tensor pipe (measured: 940 cycles per 4-MMA step with 256-512
-// cycles of tensor work).
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "elect.sync _|p, 0xffffffff;\n"
-      "selp.u32 %0, 1, 0, p;\n"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
 }
 
-// x[j] of lane l = value (row l, column j)  ->  returns for lane l the sum over the 32 rows of column l.
-// 31 shuffles instead of 32 x 5: at every halving step a lane keeps the half of the columns its bit selects
-// and sends the other half to its partner.
-__device__ __forceinline__ float warp_transpose_reduce(float (&x)[32], int lane) {
-#pragma unroll
-  for (int off = 16; off >= 1; off >>= 1) {
-    const bool up = (lane & off) != 0;
-#pragma unroll
-    for (int i = 0; i < off; ++i) {
-      const float send = up ? x[i] : x[i + off];
-      const float keep = up ? x[i + off] : x[i];
-      x[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-    }
-  }
-  return x[0];
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16_n64(float (&d)[32], uint64_t da, uint64_t db, int scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_f16_n128(float (&d)[64], uint64_t da, uint64_t db, int scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16_n128(float (&d)[64], uint64_t da, uint64_t db, int scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_f16_n256(float (&d)[128], uint64_t da, uint64_t db, int scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, %131, %132;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16_n256(float (&d)[128], uint64_t da, uint64_t db, int scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, %131, %132;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
+}
+
+template <int N, int TA, int TB, bool BF16>
+__device__ __forceinline__ void wgmma_tile(float (&d)[N / 2], uint64_t da, uint64_t db, int scale_d) {
+  if constexpr (N == 64) {
+    if constexpr (BF16) wgmma_bf16_n64<TA, TB>(d, da, db, scale_d);
+    else wgmma_f16_n64<TA, TB>(d, da, db, scale_d);
+  } else if constexpr (N == 128) {
+    if constexpr (BF16) wgmma_bf16_n128<TA, TB>(d, da, db, scale_d);
+    else wgmma_f16_n128<TA, TB>(d, da, db, scale_d);
+  } else {
+    static_assert(N == 256, "wgmma tile width");
+    if constexpr (BF16) wgmma_bf16_n256<TA, TB>(d, da, db, scale_d);
+    else wgmma_f16_n256<TA, TB>(d, da, db, scale_d);
+  }
+}
 
 // ------------------------------------------------------------------------------------------
 // descriptors
 // ------------------------------------------------------------------------------------------
-// shared-memory matrix descriptor, 128B swizzle, version 1 (Blackwell).
+// shared-memory matrix descriptor (sm_90 wgmma), 128B swizzle.
 //   K-major : rows of 128 B (64 x 16-bit along K); 8-row groups SBO bytes apart; LBO unused.
 //   MN-major: 128 B lines hold 64 MN-elements for one K index; 8 K-lines form a 1024 B group,
 //             groups SBO bytes apart; 64-element MN blocks LBO bytes apart.
+// Stage bases are 1024 B aligned, so the base-offset field stays 0; a K step inside the swizzle atom
+// advances the start address only.
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;                           // descriptor version (sm_100)
-  d |= (uint64_t)((saddr >> 7) & 0x7) << 49;        // base offset (0 for 1024 B aligned tiles)
-  d |= (uint64_t)2 << 61;                           // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                           // SWIZZLE_128B
   return d;
 }
-// instruction descriptor for kind::f16, fp32 accumulate
-__host__ __device__ inline uint32_t make_idesc(int a_bf16, int b_bf16, int a_mn_major, int b_mn_major, int M, int N) {
-  uint32_t d = 0;
-  d |= 1u << 4;                          // C format: F32
-  d |= (uint32_t)(a_bf16 ? 1 : 0) << 7;  // A format
-  d |= (uint32_t)(b_bf16 ? 1 : 0) << 10; // B format
-  d |= (uint32_t)(a_mn_major ? 1 : 0) << 15;
-  d |= (uint32_t)(b_mn_major ? 1 : 0) << 16;
-  d |= (uint32_t)(N >> 3) << 17;
-  d |= (uint32_t)(M >> 4) << 24;
-  return d;
+
+// One 64-deep K block (one ring stage) as four k16 wgmmas.  a_step / b_step: descriptor advance per k16 in
+// 16-byte units (K-major: 32 B along the row; MN-major: 16 lines of 128 B).
+template <int N, int TA, int TB, bool BF16>
+__device__ __forceinline__ void mma_k64(float (&acc)[N / 2], uint64_t da, uint64_t db, uint32_t a_step,
+                                        uint32_t b_step, bool first) {
+  wgmma_fence();
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk)
+    wgmma_tile<N, TA, TB, BF16>(acc, da + kk * a_step, db + kk * b_step, (first && kk == 0) ? 0 : 1);
+  wgmma_commit();
 }
 
 constexpr int STAGES = 4;
 constexpr int A_STAGE_BYTES = 128 * 128;   // 128 rows x 128 B
 constexpr int B_STAGE_BYTES = 256 * 128;   // up to 256 rows x 128 B
 constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
-constexpr int NUM_THREADS = 192;
+constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/ + 2048 /*column statistics*/;
+constexpr int NUM_THREADS = 384;           // producer warpgroup + two consumer warpgroups
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 
 struct TapRangesTC {
   int k_lo[NTAP], k_hi[NTAP], n_lo[NTAP], n_hi[NTAP];
@@ -212,15 +226,12 @@ struct FTcParams {
   int batch, ksplit;
   int TR, TB, TN;            // M tile = TB batches x TR rows (<= 128), N tile
   int m_tiles_per_b, b_tiles, n_tiles;
-  uint32_t idesc;
-  int dbg;                   // timing experiments only (SEGAN_B200_DEBUG): 1 skip B loads, 2 skip A loads, 4 skip stores,
-                             // 8 skip the split-K partial stores, 16 skip the finisher's partial loads
-  double* stats;             // fused BatchNorm statistics [SG_STAT_SLICES][2][nc] (CTA-pair kernel), or nullptr
-  // CTA-pair kernel only:
+  int dbg;                   // SEGAN_B200_DEBUG (bit 20: phase timeline)
+  double* stats;             // fused BatchNorm statistics [SG_STAT_SLICES][2][nc], or nullptr
   int sk_dp_tiles;           // tiles [0, sk_dp_tiles) are tile-strided; each of the rest is split along K over
-  int sk_split;              // sk_split CTA pairs
-  float* sk_ws;              // stream-K workspace [npairs][2][128][TN] fp32 (zero between launches)
-  unsigned int* sk_cnt;      // k-step counters [npairs][2][4] (zero between launches)
+  int sk_split;              // sk_split CTAs
+  float* sk_ws;              // stream-K partial sums [ctas][128 x 256] fp32
+  unsigned int* sk_cnt;      // k-step counters [leftover tiles][8 consumer warps] (zero between launches)
   void* out2;                // fused PReLU output (16-bit, out's dtype and column geometry), or nullptr
   int out2_halo;             // reflect halo rows of out2 (its buffer has out_rows + 2 * out2_halo rows per batch element)
   const float* slope; int slope_mod;
@@ -230,12 +241,9 @@ struct FTcParams {
 struct SharedCtl {
   uint64_t full[STAGES];
   uint64_t empty[STAGES];
-  uint64_t tmem_full[8];      // up to 512 / TN accumulator stages (2 x 256 ... 8 x 64 columns)
-  uint64_t tmem_empty[8];
-  uint32_t tmem_base;
 };
 
-// number of 64-channel K steps a tile with N range [n0, n0+TN) executes for K-split `ks`
+// number of 64-channel K steps a tile with N range [n0, n0+TN) executes for interleaved K split `ks`
 __device__ __forceinline__ int f_num_steps(const FTcParams& p, int n0, int ks) {
   int total = 0;
   for (int d = p.d_lo; d <= p.d_hi; ++d) {
@@ -246,285 +254,28 @@ __device__ __forceinline__ int f_num_steps(const FTcParams& p, int n0, int ks) {
   return p.ksplit == 1 ? total : (total - ks + p.ksplit - 1) / p.ksplit;
 }
 
-// ------------------------------------------------------------------------------------------
-// form F:  out[b,m,n] = bias + sum_d sum_kc A[b,m+d,kc] * Wp[d+4][n][kc]
-//   UMMA: M = 128 (rows: TB batches x TR rows), N = TN output channels, K = 64-channel blocks.
-// ------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-tapgemm_f_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
-             const __grid_constant__ CUtensorMap tmW, const FTcParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  SharedCtl* ctl = reinterpret_cast<SharedCtl*>(smem + STAGES * STAGE_BYTES);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmA0); prefetch_tmap(&tmA1); prefetch_tmap(&tmW);
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&ctl->full[s], 1); mbar_init(&ctl->empty[s], 1); }
-    for (int i = 0; i < 8; ++i) { mbar_init(&ctl->tmem_full[i], 1); mbar_init(&ctl->tmem_empty[i], 128); }
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc(&ctl->tmem_base, 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = ctl->tmem_base;
-
-  const int m_tiles = p.m_tiles_per_b * p.b_tiles;
-  const int total_tiles = m_tiles * p.n_tiles * p.ksplit;
-  const uint32_t a_bytes = (uint32_t)p.TR * p.TB * 128u;
-  const uint32_t b_bytes = (uint32_t)p.TN * 128u;
-  const int nacc = 512 / p.TN;     // accumulator stages in TMEM: short-K tiles are bound by this ping-pong depth
-
-  if (warp == 0) {
-    // ================= TMA producer =================
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int mt = tile % m_tiles;
-        const int rest = tile / m_tiles;
-        const int ks = rest % p.ksplit;
-        const int nt = rest / p.ksplit;
-        const int b0 = (mt / p.m_tiles_per_b) * p.TB;
-        const int m0 = p.m_lo + (mt % p.m_tiles_per_b) * p.TR;
-        const int n0 = p.n_lo + nt * p.TN;
-        int step = 0;
-        for (int d = p.d_lo; d <= p.d_hi; ++d) {
-          const int ti = d + 4;
-          if (n0 + p.TN <= p.tr.n_lo[ti] || n0 >= p.tr.n_hi[ti]) continue;
-          for (int k0 = p.tr.k_lo[ti]; k0 < p.tr.k_hi[ti]; k0 += 64, ++step) {
-            if (p.ksplit > 1 && step % p.ksplit != ks) continue;
-            mbar_wait(&ctl->empty[stage], phase ^ 1);
-            uint8_t* sa = smem + stage * STAGE_BYTES;
-            uint8_t* sb = sa + A_STAGE_BYTES;
-            mbar_expect_tx(&ctl->full[stage], ((p.dbg & 2) ? 0u : a_bytes) + ((p.dbg & 1) ? 0u : b_bytes));
-            if (!(p.dbg & 2)) {
-              if (k0 < p.a0_c) tma_load_3d(sa, &tmA0, &ctl->full[stage], k0, m0 + d + p.a_halo, b0);
-              else tma_load_3d(sa, &tmA1, &ctl->full[stage], k0 - p.a0_c, m0 + d + p.a_halo, b0);
-            }
-            if (!(p.dbg & 1)) tma_load_2d(sb, &tmW, &ctl->full[stage], k0, (ti - p.w_tap0) * p.nc + n0);
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ================= MMA issuer: warp-uniform loop, one elected lane issues =================
-    {
-      int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int rest = tile / m_tiles;
-        const int ks = rest % p.ksplit;
-        const int nt = rest / p.ksplit;
-        const int n0 = p.n_lo + nt * p.TN;
-        mbar_wait(&ctl->tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(acc * p.TN);
-        // the issuer only needs the NUMBER of K steps (the producer decides what they contain)
-        const int nsteps = f_num_steps(p, n0, ks);
-        const uint32_t smem0 = smem_u32(smem);
-        for (int i = 0; i < nsteps; ++i) {
-          mbar_wait(&ctl->full[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem0 + (uint32_t)stage * STAGE_BYTES;
-          const uint64_t adesc = make_smem_desc(sa, 16, 1024);
-          const uint64_t bdesc = make_smem_desc(sa + A_STAGE_BYTES, 16, 1024);
-          if (elect_one()) {
-            umma_f16(tmem_d, adesc, bdesc, p.idesc, i > 0 ? 1u : 0u);
-            umma_f16(tmem_d, adesc + 2, bdesc + 2, p.idesc, 1u);
-            umma_f16(tmem_d, adesc + 4, bdesc + 4, p.idesc, 1u);
-            umma_f16(tmem_d, adesc + 6, bdesc + 6, p.idesc, 1u);
-            umma_commit(&ctl->empty[stage]);   // frees the smem slot when these MMAs retire
-          }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        if (elect_one()) umma_commit(&ctl->tmem_full[acc]);     // accumulator complete
-        __syncwarp();
-        if (++acc == nacc) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else {
-    // ================= epilogue (warps 2..5) =================
-    const int quad = warp & 3;                  // TMEM lane quadrant this warp may access
-    const int row = quad * 32 + lane;           // accumulator row = tile row
-    int acc = 0; uint32_t acc_phase = 0;
-    const int out_buf_rows = p.out_rows + 2 * p.out_halo;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const int mt = tile % m_tiles;
-      const int rest = tile / m_tiles;
-      const int ks = rest % p.ksplit;
-      const int nt = rest / p.ksplit;
-      const int b0 = (mt / p.m_tiles_per_b) * p.TB;
-      const int m0 = p.m_lo + (mt % p.m_tiles_per_b) * p.TR;
-      const int n0 = p.n_lo + nt * p.TN;
-      const int tb = row / p.TR, tr = row % p.TR;
-      const int b = b0 + tb, m = m0 + tr;
-      const bool valid = (tb < p.TB) && (b < p.batch) && (m < p.m_hi);
-      mbar_wait(&ctl->tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * p.TN);
-      const int64_t obase = ((int64_t)b * out_buf_rows + (m + p.out_halo)) * p.out_ld + (n0 - p.n_lo + p.out_col0);
-      for (int c0 = 0; c0 < p.TN; c0 += 32) {
-        uint32_t r[32];
-        tmem_ld32(taddr + (uint32_t)c0, r);
-        tmem_ld_wait();
-        if (valid && !(p.dbg & 4)) {
-          float v[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-          if (p.bias != nullptr && ks == 0) {
-            // bias_mod is a multiple of 64 and the chunk is 32-aligned: one modulo per chunk
-            // (scalar loads: bias vectors are 4-byte-aligned views of the flat parameter buffer)
-            const float* bp = p.bias + ((n0 + c0) % p.bias_mod);
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] += __ldg(bp + j);
-          }
-          if (p.out_dtype == SG_F32) {
-            float* o = reinterpret_cast<float*>(p.out) + obase + c0;
-            if (p.ksplit == 1) {
-#pragma unroll
-              for (int j = 0; j < 32; j += 4)
-                *reinterpret_cast<float4*>(o + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) red_add_v4(o + j, v[j], v[j + 1], v[j + 2], v[j + 3]);
-            }
-          } else {
-            uint32_t pk[16];
-            if (p.out_dtype == SG_F16) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) {
-                pk[j] = pack_half2_sat(v[2 * j], v[2 * j + 1]);
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) {
-                __nv_bfloat162 h = __floats2bfloat162_rn(v[2 * j], v[2 * j + 1]);
-                pk[j] = *reinterpret_cast<uint32_t*>(&h);
-              }
-            }
-            uint4* o = reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.out) + obase + c0);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) o[j] = make_uint4(pk[4 * j], pk[4 * j + 1], pk[4 * j + 2], pk[4 * j + 3]);
-          }
-        }
-      }
-      tc_fence_before();
-      mbar_arrive(&ctl->tmem_empty[acc]);
-      if (++acc == nacc) { acc = 0; acc_phase ^= 1; }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-// ------------------------------------------------------------------------------------------
-// form F on CTA pairs (tcgen05 cta_group::2): two CTAs of a cluster compute a 256 x TN tile.
-// Each CTA stages its own 128 rows of A and HALF of the weight tile; the leader's single thread
-// issues M = 256 UMMAs that read both CTAs' shared memory, so per-SM shared-memory traffic per
-// MMA drops from 12 KB to 8 KB and the weight tile is fetched from L2 once per pair.
-// (Measured on the 1-CTA kernel: UMMA operand reads + TMA fill ~ 192 B/clk against the 128 B/clk
-// shared-memory port capped the tensor pipe at 66 %, profiles/r1_v1_ncu_tapgemm_f.md.)
-// ------------------------------------------------------------------------------------------
-constexpr int STAGES2 = 6;
-constexpr int B2_STAGE_BYTES = 128 * 128;            // half of a 256-row weight tile
-constexpr int STAGE2_BYTES = A_STAGE_BYTES + B2_STAGE_BYTES;
-constexpr int SMEM2_BYTES = STAGES2 * STAGE2_BYTES + 1024 + 256 + 2048;   // + per-CTA column statistics [2][256] fp32
-constexpr uint32_t PEER_MASK = 0xFEFFFFFFu;          // shared::cluster address of the even (leader) CTA
-
-struct SharedCtl2 {
-  uint64_t full[STAGES2];
-  uint64_t empty[STAGES2];
-  uint64_t tmem_full[8];      // up to 512 / TN accumulator stages (2 x 256 ... 8 x 64 columns)
-  uint64_t tmem_empty[8];
-  uint32_t tmem_base;
-};
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tma_load_2d_pair(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar) & PEER_MASK), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_pair(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1,
-                                                 int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar) & PEER_MASK), "r"(c0), "r"(c1),
-      "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols));
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::);
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols));
-}
-__device__ __forceinline__ void umma_f16_pair(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive (count 1) on the same barrier in BOTH CTAs of the pair when the issued MMAs retire
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"((uint16_t)3)
-      : "memory");
-}
-// plain arrive on the LEADER's copy of a barrier
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & PEER_MASK) : "memory");
-}
-
-// ---- work decomposition of tapgemm_f_tc2 ------------------------------------------------------------
-// Tiles [0, sk_dp_tiles) are scheduled tile-strided over the CTA pairs as before.  With batch 300 nearly every
-// layer has a tile count just above a multiple of the 74 pairs (300 = 4 x 75: 76, 150, 300, 600, 1200 tiles), so
-// the last wave ran 2-16 tiles on 74 pairs.  Each leftover tile [sk_dp_tiles, total) is therefore split along K
-// over sk_split pairs (pair p takes k-range p % sk_split of leftover tile p / sk_split): every one of them adds its
-// fp32 partial sums into a workspace tile (vector red) and bumps the tile's k-step counter; the warp whose bump
-// completes the count reads the sums back, applies bias / conversion, stores, and leaves workspace and counter
-// zeroed for the next launch.  No pair ever waits for another one.  The split factor is chosen by the host: the
-// partial sums cost L2 atomics in proportion to sk_split, the tail shrinks as 1 / sk_split (tapgemm_f_tc_launch).
+// ---- work decomposition of tapgemm_f_tc -------------------------------------------------------------
+// Tiles [0, sk_dp_tiles) are scheduled tile-strided over the CTAs.  With batch 300 many layers have a tile count
+// just above a multiple of the CTA count, so the last wave ran a few tiles on an otherwise idle GPU.  Each leftover
+// tile [sk_dp_tiles, total) is therefore split along K over sk_split CTAs (CTA c takes k-range c % sk_split of
+// leftover tile c / sk_split): every one of them stores its fp32 partial sums into its own workspace slot and bumps
+// the tile's counter; the warp whose bump completes the count adds the slots up in slot order (deterministic),
+// applies bias / conversion, stores, and leaves the counter zeroed for the next launch.  No CTA ever waits for
+// another one.  The split factor is chosen by the host: the partial sums cost L2 traffic in proportion to sk_split,
+// the tail shrinks as 1 / sk_split (tapgemm_f_tc_launch).
 struct Piece {
-  int tile;      // tile index (mp fastest, then ksplit, then nt)
-  int mp, rest;  // tile % m_pairs, tile / m_pairs (tracked incrementally: no division per tile)
+  int tile;      // tile index (mt fastest, then ksplit, then nt)
+  int mt, rest;  // tile % m_tiles, tile / m_tiles (tracked incrementally: no division per tile)
   int kb, ke;    // k-step range [kb, ke) of the tile's `total` steps (split-K pieces; whole tile otherwise)
   int total;
 };
 
-// The waveform-end GEMMs have ONE k-step per tile and 65 tiles per CTA: whatever a role executes per tile is their
-// critical path (ncu, profiles/r2_v1_ncu_tapgemm.md: ~2400 warp instructions per tile and epilogue warp, a dozen
-// integer divisions among them, made a 314 MB pass take 127 us).  The iterator therefore advances (mp, rest) by
-// addition and caches the k-step count per N tile; the roles hoist everything that does not depend on the tile.
-// SEGAN_B200_DEBUG bit 20: phase timeline of tapgemm_f_tc2 (globaltimer ns; epilogue warp 2 / lane 0 of every CTA):
+// SEGAN_B200_DEBUG bit 20: phase timeline of tapgemm_f_tc (globaltimer ns; first consumer thread of every CTA):
 // [cta][0] = kernel start, then per piece: accumulator ready, epilogue done, (split tiles) finisher done; last = exit.
 // Read back with sg_debug_timeline (diagnostics only).
 constexpr int TL_SLOTS = 32;
-__device__ unsigned long long g_tc2_timeline[160 * TL_SLOTS];
+constexpr int TL_CTAS = 160;
+__device__ unsigned long long g_tc_timeline[TL_CTAS * TL_SLOTS];
 __device__ __forceinline__ unsigned long long gtime_ns() {
   unsigned long long t;
   asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
@@ -532,8 +283,8 @@ __device__ __forceinline__ unsigned long long gtime_ns() {
 }
 
 struct PieceIter {
-  int m_pairs, npairs, dp_end, total_tiles, pair_id;
-  int next_dp, cur_mp, cur_rest;
+  int m_tiles, nctas, dp_end, total_tiles, cta;
+  int next_dp, cur_mt, cur_rest;
   int cache_rest, cache_steps;
   bool sk_done;
 
@@ -545,31 +296,30 @@ struct PieceIter {
     }
     return cache_steps;
   }
-  __device__ __forceinline__ void init(const FTcParams& p, int m_pairs_, int total_tiles_, int pair_id_, int npairs_) {
-    m_pairs = m_pairs_; npairs = npairs_; total_tiles = total_tiles_; pair_id = pair_id_;
+  __device__ __forceinline__ void init(const FTcParams& p, int m_tiles_, int total_tiles_, int cta_, int nctas_) {
+    m_tiles = m_tiles_; nctas = nctas_; total_tiles = total_tiles_; cta = cta_;
     dp_end = p.sk_dp_tiles < total_tiles_ ? p.sk_dp_tiles : total_tiles_;
-    next_dp = pair_id_;
-    cur_rest = pair_id_ / m_pairs_;
-    cur_mp = pair_id_ - cur_rest * m_pairs_;
+    next_dp = cta_;
+    cur_rest = cta_ / m_tiles_;
+    cur_mt = cta_ - cur_rest * m_tiles_;
     cache_rest = -1; cache_steps = 0;
     sk_done = false;
   }
-  template <bool SKF>
   __device__ __forceinline__ bool next(const FTcParams& p, Piece& pc) {
     if (next_dp < dp_end) {
-      pc.tile = next_dp; pc.mp = cur_mp; pc.rest = cur_rest;
+      pc.tile = next_dp; pc.mt = cur_mt; pc.rest = cur_rest;
       pc.kb = 0; pc.total = pc.ke = steps_of_rest(p, cur_rest);
-      next_dp += npairs;
-      cur_mp += npairs;
-      while (cur_mp >= m_pairs) { cur_mp -= m_pairs; ++cur_rest; }
+      next_dp += nctas;
+      cur_mt += nctas;
+      while (cur_mt >= m_tiles) { cur_mt -= m_tiles; ++cur_rest; }
       return true;
     }
-    if (!SKF || sk_done || dp_end >= total_tiles) return false;
+    if (sk_done || dp_end >= total_tiles) return false;
     sk_done = true;
-    const int t = dp_end + pair_id / p.sk_split;
+    const int t = dp_end + cta / p.sk_split;
     if (t >= total_tiles) return false;
-    const int part = pair_id % p.sk_split;
-    pc.tile = t; pc.rest = t / m_pairs; pc.mp = t - pc.rest * m_pairs;
+    const int part = cta % p.sk_split;
+    pc.tile = t; pc.rest = t / m_tiles; pc.mt = t - pc.rest * m_tiles;
     const int s = steps_of_rest(p, pc.rest);
     pc.total = s;
     pc.kb = (int)((long long)s * part / p.sk_split);
@@ -578,154 +328,175 @@ struct PieceIter {
   }
 };
 
-// v[j] += bias[(n_abs + j) % bias_mod], 16-byte loads (bias_mod is a multiple of 64, the chunk 32-aligned, the vector
-// a 16-byte aligned view)
 __device__ __forceinline__ int f_mod(int x, int mod, int mask) { return mask >= 0 ? (x & mask) : (x % mod); }
 
-__device__ __forceinline__ void f_add_bias(const FTcParams& p, float (&v)[32], int n_abs) {
-  const float4* bp = reinterpret_cast<const float4*>(p.bias + f_mod(n_abs, p.bias_mod, p.bias_mask));
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const float4 t = __ldg(bp + j);
-    v[4 * j] += t.x; v[4 * j + 1] += t.y; v[4 * j + 2] += t.z; v[4 * j + 3] += t.w;
-  }
+__device__ __forceinline__ uint32_t pack2(float x, float y, int dtype) {
+  if (dtype == SG_F16) return pack_half2_sat(x, y);
+  __nv_bfloat162 h = __floats2bfloat162_rn(x, y);
+  return *reinterpret_cast<uint32_t*>(&h);
 }
 
-// one 32-column chunk of an output row: bias / conversion / stores, and the fused second output
+// Two adjacent columns (n_abs, n_abs + 1) of one output row: conversion / stores, and the fused second output
 //   out2[b][row2][n] = PReLU(v) (16-bit), the consumer-ready activation of the Generator's conv / deconv blocks
 //   (modules.py:99-101,139-141: no norm layer between the contraction and the PReLU), written next to the raw
 //   pre-activation (`out`, the skip connection's source, generator.py:185,191) with its reflect halo
 //   (modules.py:92-98): position m also lands on its mirror row when it lies within `out2_halo` of an end.
-template <bool ACF>
-__device__ __forceinline__ void f_store_chunk(const FTcParams& p, float (&v)[32], int64_t obase, int c0, int n_abs,
-                                              bool atomic, int64_t o2base, int64_t o2mirror) {
+// x / y return the values stored into `out` (the BatchNorm statistics describe them).
+__device__ __forceinline__ void f_store2(const FTcParams& p, float& x, float& y, int64_t o, int n_abs, bool atomic,
+                                         int64_t o2, int64_t o2mirror) {
   if (p.out_dtype == SG_F32) {
-    float* o = reinterpret_cast<float*>(p.out) + obase + c0;
-    if (!atomic) {
-#pragma unroll
-      for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(o + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-    } else {
-#pragma unroll
-      for (int j = 0; j < 32; j += 4) red_add_v4(o + j, v[j], v[j + 1], v[j + 2], v[j + 3]);
-    }
+    float* dst = reinterpret_cast<float*>(p.out) + o;
+    if (atomic) red_add_v2(dst, x, y);
+    else *reinterpret_cast<float2*>(dst) = make_float2(x, y);
     return;
   }
-  uint32_t pk[16];
-  float sl[32];
-  if (ACF && p.slope != nullptr) {
-    // 16-byte loads: slope / bias vectors are 16-byte aligned views and the chunk is 32-aligned
-    const float4* sp = reinterpret_cast<const float4*>(p.slope + f_mod(n_abs, p.slope_mod, p.slope_mask));
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float4 t = __ldg(sp + j);
-      sl[4 * j] = t.x; sl[4 * j + 1] = t.y; sl[4 * j + 2] = t.z; sl[4 * j + 3] = t.w;
+  float s0 = 0.f, s1 = 0.f;
+  if (p.slope != nullptr) {
+    const float* sp = p.slope + f_mod(n_abs, p.slope_mod, p.slope_mask);    // slope_mod is even: no wrap inside the pair
+    s0 = __ldg(sp); s1 = __ldg(sp + 1);
+    if (p.out2 == nullptr) {   // PReLU applied to the (only) output: blocks whose pre-activation nobody reads
+      x = x > 0.f ? x : s0 * x;
+      y = y > 0.f ? y : s1 * y;
     }
   }
-  if (ACF && p.out2 == nullptr && p.slope != nullptr) {
-    // PReLU applied to the (only) output: blocks whose pre-activation nobody reads (inference decoder)
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = v[j] > 0.f ? v[j] : sl[j] * v[j];
+  *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.out) + o) = pack2(x, y, p.out_dtype);
+  if (p.out2 != nullptr) {
+    const uint32_t a = pack2(x > 0.f ? x : s0 * x, y > 0.f ? y : s1 * y, p.out_dtype);
+    *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.out2) + o2) = a;
+    if (o2mirror >= 0) *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.out2) + o2mirror) = a;
   }
-  if (p.out_dtype == SG_F16) {
+}
+
+__device__ __forceinline__ float round_as_stored(float x, int dtype) {
+  if (dtype == SG_F16) return __half2float(__float2half_rn(x));
+  if (dtype == SG_BF16) return __bfloat162float(__float2bfloat16_rn(x));
+  return x;
+}
+
+// Epilogue of one consumer thread: wgmma accumulator fragment -> bias / conversion / stores (+ BatchNorm column
+// statistics into shared memory).  Fragment layout of m64nN: consumer warp cw (0..7) owns tile rows 16 cw + lane/4
+// and 16 cw + 8 + lane/4; register 4j + 2h + e holds column 8j + 2(lane%4) + e of the h-th of those rows.
+template <int TN>
+__device__ __forceinline__ void f_epilogue(const FTcParams& p, float (&acc)[TN / 2], int mt, int n0, int ks, int ctid,
+                                           float* colstat) {
+  const int lane = ctid & 31, cw = ctid >> 5;
+  const int out_buf_rows = p.out_rows + 2 * p.out_halo;
+  const int out2_buf_rows = p.out_rows + 2 * p.out2_halo;
+  const int mtb = p.m_tiles_per_b == 1 ? mt : mt / p.m_tiles_per_b;
+  const int b0 = mtb * p.TB;
+  const int m0 = p.m_lo + (mt - mtb * p.m_tiles_per_b) * p.TR;
+  const int col0 = n0 - p.n_lo + p.out_col0 + 2 * (lane & 3);
+  int64_t obase[2], o2base[2], o2mirror[2];
+  bool valid[2];
 #pragma unroll
-    for (int j = 0; j < 16; ++j) pk[j] = pack_half2_sat(v[2 * j], v[2 * j + 1]);
-  } else {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      __nv_bfloat162 h = __floats2bfloat162_rn(v[2 * j], v[2 * j + 1]);
-      pk[j] = *reinterpret_cast<uint32_t*>(&h);
+  for (int h = 0; h < 2; ++h) {
+    const int r = cw * 16 + (lane >> 2) + 8 * h;
+    const int tb = r / p.TR, tr = r - tb * p.TR;
+    const int b = b0 + tb, m = m0 + tr;
+    valid[h] = (tb < p.TB) && (b < p.batch) && (m < p.m_hi);
+    obase[h] = ((int64_t)b * out_buf_rows + (m + p.out_halo)) * p.out_ld + col0;
+    o2base[h] = 0; o2mirror[h] = -1;
+    if (p.out2 != nullptr) {
+      const int64_t rb = (int64_t)b * out2_buf_rows + p.out2_halo;
+      o2base[h] = (rb + m) * p.out_ld + col0;
+      if (p.out2_halo > 0) {
+        int mm = 0;
+        bool has = false;
+        if (m >= 1 && m <= p.out2_halo) { mm = -m; has = true; }
+        else if (m >= p.out_rows - 1 - p.out2_halo && m <= p.out_rows - 2) { mm = 2 * (p.out_rows - 1) - m; has = true; }
+        if (has) o2mirror[h] = (rb + mm) * p.out_ld + col0;
+      }
     }
   }
-  uint4* o = reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.out) + obase + c0);
+  const bool add_bias = p.bias != nullptr && ks == 0;
+  const bool atomic = p.ksplit > 1;
 #pragma unroll
-  for (int j = 0; j < 4; ++j) o[j] = make_uint4(pk[4 * j], pk[4 * j + 1], pk[4 * j + 2], pk[4 * j + 3]);
-  if (ACF && p.out2 != nullptr) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const float x0 = v[2 * j], x1 = v[2 * j + 1];
-      const float y0 = x0 > 0.f ? x0 : sl[2 * j] * x0;
-      const float y1 = x1 > 0.f ? x1 : sl[2 * j + 1] * x1;
-      pk[j] = pack_half2_sat(y0, y1);
+  for (int j = 0; j < TN / 8; ++j) {
+    const int c = 8 * j + 2 * (lane & 3);
+    float bx = 0.f, by = 0.f;
+    if (add_bias) {    // bias_mod is a multiple of 64: no wrap inside the pair
+      const float* bp = p.bias + f_mod(n0 + c, p.bias_mod, p.bias_mask);
+      bx = __ldg(bp); by = __ldg(bp + 1);
     }
-    uint4* o2 = reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.out2) + o2base + c0);
+    float sx = 0.f, sy = 0.f, qx = 0.f, qy = 0.f;
 #pragma unroll
-    for (int j = 0; j < 4; ++j) o2[j] = make_uint4(pk[4 * j], pk[4 * j + 1], pk[4 * j + 2], pk[4 * j + 3]);
-    if (o2mirror >= 0) {
-      uint4* o3 = reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.out2) + o2mirror + c0);
+    for (int h = 0; h < 2; ++h) {
+      float x = acc[4 * j + 2 * h] + bx, y = acc[4 * j + 2 * h + 1] + by;
+      if (valid[h]) {
+        f_store2(p, x, y, obase[h] + 8 * j, n0 + c, atomic, o2base[h] + 8 * j, o2mirror[h] >= 0 ? o2mirror[h] + 8 * j : -1);
+        x = round_as_stored(x, p.out_dtype);
+        y = round_as_stored(y, p.out_dtype);
+        sx += x; sy += y; qx += x * x; qy += y * y;
+      }
+    }
+    if (p.stats != nullptr) {            // uniform branch: the reduction is warp-collective
 #pragma unroll
-      for (int j = 0; j < 4; ++j) o3[j] = make_uint4(pk[4 * j], pk[4 * j + 1], pk[4 * j + 2], pk[4 * j + 3]);
+      for (int o = 4; o < 32; o <<= 1) {
+        sx += __shfl_xor_sync(0xffffffffu, sx, o);
+        sy += __shfl_xor_sync(0xffffffffu, sy, o);
+        qx += __shfl_xor_sync(0xffffffffu, qx, o);
+        qy += __shfl_xor_sync(0xffffffffu, qy, o);
+      }
+      if (lane < 4) {
+        atomicAdd(colstat + c, sx);
+        atomicAdd(colstat + c + 1, sy);
+        atomicAdd(colstat + 256 + c, qx);
+        atomicAdd(colstat + 256 + c + 1, qy);
+      }
     }
   }
 }
 
-// 10 warps: TMA producer, MMA issuer and EIGHT epilogue warps -- two per TMEM lane quadrant, taking alternate
-// 32-column chunks.  The layers with one or two k-steps per tile (the waveform-end GEMMs, K = 64) are bound by the
-// epilogue's instruction issue, not by the tensor pipe or HBM (profiles/r2_calls_*.txt: 157 MB in + 157 MB out took
-// 141 us with four warps).
-constexpr int NUM_THREADS2 = 320;
-__device__ __forceinline__ void epi2_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
-
-// FEAT: compile-time feature set (bit 0 split-K pieces, 1 fused BatchNorm statistics, 2 fused PReLU / second output,
-// 3 interleaved k-split with fp32 atomics; 15 = everything + diagnostics).  The waveform-end launches run ONE k-step per
-// tile and 65 tiles per CTA: their epilogue warps were issuing at ~8 cycles per instruction through a 5500-instruction
-// kernel (timeline: 1.65 us per tile and warp for a 32 x 32 chunk), so the launch picks the leanest instantiation.
-template <int FEAT>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NUM_THREADS2, 1)
-tapgemm_f_tc2(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
-              const __grid_constant__ CUtensorMap tmW, const FTcParams p) {
-  constexpr bool SKF = (FEAT & 1) != 0, STF = (FEAT & 2) != 0, ACF = (FEAT & 4) != 0, KSF = (FEAT & 8) != 0;
-  constexpr bool DBG = FEAT == 15;
+// ------------------------------------------------------------------------------------------
+// form F:  out[b,m,n] = bias + sum_d sum_kc A[b,m+d,kc] * Wp[d+4][n][kc]
+//   wgmma: M = 128 (rows: TB batches x TR rows; 64 per consumer warpgroup), N = TN output channels,
+//   K = 64-channel blocks.  Optional: interleaved K split into fp32 (ksplit > 1, vector red), stream-K tail,
+//   fused BatchNorm statistics, fused PReLU / second output.
+// ------------------------------------------------------------------------------------------
+// BF16: operand format (bf16 / fp16), a template parameter so that each wgmma has one fixed form
+template <int TN, bool BF16>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+tapgemm_f_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
+             const __grid_constant__ CUtensorMap tmW, const FTcParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  SharedCtl2* ctl = reinterpret_cast<SharedCtl2*>(smem + STAGES2 * STAGE2_BYTES);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
+  SharedCtl* ctl = reinterpret_cast<SharedCtl*>(smem + STAGES * STAGE_BYTES);
+  float* colstat = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES + 256);      // [2][256]
+  const int wg = threadIdx.x >> 7;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmA0); prefetch_tmap(&tmA1); prefetch_tmap(&tmW);
-    for (int s = 0; s < STAGES2; ++s) { mbar_init(&ctl->full[s], 1); mbar_init(&ctl->empty[s], 1); }
-    for (int i = 0; i < 8; ++i) { mbar_init(&ctl->tmem_full[i], 1); mbar_init(&ctl->tmem_empty[i], 16); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&ctl->full[s], 1); mbar_init(&ctl->empty[s], 2); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc_pair(&ctl->tmem_base, 512);
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = ctl->tmem_base;
+  if (p.stats != nullptr)
+    for (int c = threadIdx.x; c < 512; c += NUM_THREADS) colstat[c] = 0.f;
+  __syncthreads();
 
   const int m_tiles = p.m_tiles_per_b * p.b_tiles;
-  const int m_pairs = (m_tiles + 1) / 2;
-  const int total_tiles = m_pairs * p.n_tiles * p.ksplit;
-  const int npairs = gridDim.x / 2;
-  const int pair_id = blockIdx.x / 2;
-  const int half_n = p.TN / 2;
+  const int total_tiles = m_tiles * p.n_tiles * p.ksplit;
   const uint32_t a_bytes = (uint32_t)p.TR * p.TB * 128u;
-  const uint32_t b_bytes = (uint32_t)half_n * 128u;
-  const int nacc = 512 / p.TN;
+  const uint32_t b_bytes = (uint32_t)TN * 128u;
   PieceIter it;
-  it.init(p, m_pairs, total_tiles, pair_id, npairs);
+  it.init(p, m_tiles, total_tiles, blockIdx.x, gridDim.x);
   Piece pc;
 
-  if (warp == 0) {
-    // ================= TMA producer (both CTAs) =================
-    if (lane < 2) {
+  if (wg == 0) {
+    // ================= TMA producer =================
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (threadIdx.x == 0) {
       int stage = 0; uint32_t phase = 0;
-      while (it.template next<SKF>(p, pc)) {
-        const int ks = (!KSF || p.ksplit == 1) ? 0 : pc.rest % p.ksplit;
-        const int nt = (!KSF || p.ksplit == 1) ? pc.rest : pc.rest / p.ksplit;
-        const int mt = 2 * pc.mp + (int)rank;
-        const int mtb = p.m_tiles_per_b == 1 ? mt : mt / p.m_tiles_per_b;
+      while (it.next(p, pc)) {
+        const int ks = p.ksplit == 1 ? 0 : pc.rest % p.ksplit;
+        const int nt = p.ksplit == 1 ? pc.rest : pc.rest / p.ksplit;
+        const int mtb = p.m_tiles_per_b == 1 ? pc.mt : pc.mt / p.m_tiles_per_b;
         const int b0 = mtb * p.TB;
-        const int m0 = p.m_lo + (mt - mtb * p.m_tiles_per_b) * p.TR;
+        const int m0 = p.m_lo + (pc.mt - mtb * p.m_tiles_per_b) * p.TR;
         const int n0 = p.n_lo + nt * p.TN;
-        // k-steps [kb, ke) of the tile's (tap, k-block) sequence.  A split-K piece JUMPS to its first step: walking
-        // there one (tap, k-block) at a time cost ~0.12 us per skipped step (two dependent constant-bank loads per
-        // iteration), i.e. the 7th piece of a 248-step tile started 25 us late (profiles/r2_tc2_timeline.txt).
-        // An interleaved k-split tile (ksplit > 1: the fc.0 GEMM, K = 16384) takes every ksplit-th (tap, k-block)
-        // starting at block ks: it strides there as well -- the per-block `step % ksplit` test was a division per
-        // skipped block (256 blocks walked for 16 loaded).
-        const bool interleaved = KSF && p.ksplit > 1;
+        // k-steps [kb, ke) of the tile's (tap, k-block) sequence; a split-K piece jumps to its first step.  An
+        // interleaved k-split tile (ksplit > 1: the fc.0 GEMM, K = 16384) takes every ksplit-th (tap, k-block)
+        // starting at block ks.
+        const bool interleaved = p.ksplit > 1;
         int step = 0, sel = 0;              // step: first (tap, k-block) index of the current tap; sel: steps passed
         int skip = interleaved ? 0 : pc.kb;
         int next_sel = ks;                  // interleaved: global index of the next block this tile takes
@@ -746,479 +517,126 @@ tapgemm_f_tc2(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ 
           }
           for (; k0 < khi; k0 += kstride) {
             if (!interleaved) {
-              const int mine = sel++;
-              if (mine >= pc.ke) break;
+              if (sel++ >= pc.ke) break;
             } else {
               next_sel += p.ksplit;
             }
             mbar_wait(&ctl->empty[stage], phase ^ 1);
-            uint8_t* sa = smem + stage * STAGE2_BYTES;
-            if (leader && lane == 0) mbar_expect_tx(&ctl->full[stage], 2u * (a_bytes + b_bytes));
-            // lane 0: this CTA's A box; lane 1: its half of the weight box -- one warp instruction
-            const bool in0 = k0 < p.a0_c;
-            const CUtensorMap* map = lane == 0 ? (in0 ? &tmA0 : &tmA1) : &tmW;
-            const int c0 = (lane == 0 && !in0) ? k0 - p.a0_c : k0;
-            const int c1 = lane == 0 ? m0 + d + p.a_halo : (ti - p.w_tap0) * p.nc + n0 + (int)rank * half_n;
-            const int c2 = lane == 0 ? b0 : 0;
-            tma_load_3d_pair(lane == 0 ? sa : sa + A_STAGE_BYTES, map, &ctl->full[stage], c0, c1, c2);
-            if (++stage == STAGES2) { stage = 0; phase ^= 1; }
+            uint8_t* sa = smem + stage * STAGE_BYTES;
+            mbar_expect_tx(&ctl->full[stage], a_bytes + b_bytes);
+            if (k0 < p.a0_c) tma_load_3d(sa, &tmA0, &ctl->full[stage], k0, m0 + d + p.a_halo, b0);
+            else tma_load_3d(sa, &tmA1, &ctl->full[stage], k0 - p.a0_c, m0 + d + p.a_halo, b0);
+            tma_load_2d(sa + A_STAGE_BYTES, &tmW, &ctl->full[stage], k0, (ti - p.w_tap0) * p.nc + n0);
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
           }
           step += nk;
         }
       }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer (leader CTA only) =================
-    if (leader) {      // warp-uniform loop, one elected lane issues (see elect_one)
-      int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      const uint32_t smem0 = smem_u32(smem);
-      while (it.template next<SKF>(p, pc)) {
-        mbar_wait(&ctl->tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(acc * p.TN);
-        const int nsteps = pc.ke - pc.kb;
-        for (int i = 0; i < nsteps; ++i) {
-          mbar_wait(&ctl->full[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem0 + (uint32_t)stage * STAGE2_BYTES;
-          const uint64_t adesc = make_smem_desc(sa, 16, 1024);
-          const uint64_t bdesc = make_smem_desc(sa + A_STAGE_BYTES, 16, 1024);
-          if (elect_one()) {
-            umma_f16_pair(tmem_d, adesc, bdesc, p.idesc, i > 0 ? 1u : 0u);
-            umma_f16_pair(tmem_d, adesc + 2, bdesc + 2, p.idesc, 1u);
-            umma_f16_pair(tmem_d, adesc + 4, bdesc + 4, p.idesc, 1u);
-            umma_f16_pair(tmem_d, adesc + 6, bdesc + 6, p.idesc, 1u);
-            umma_commit_pair(&ctl->empty[stage]);     // frees the slot in both CTAs
-          }
-          __syncwarp();
-          if (++stage == STAGES2) { stage = 0; phase ^= 1; }
-        }
-        if (elect_one()) umma_commit_pair(&ctl->tmem_full[acc]);
-        __syncwarp();
-        if (++acc == nacc) { acc = 0; acc_phase ^= 1; }
-      }
+    return;
+  }
+
+  // ================= consumers (warpgroups 1, 2): MMA + epilogue =================
+  setmaxnreg_inc<CONSUMER_REGS>();
+  const int ctid = threadIdx.x - 128;              // 0..255
+  const int cwg = wg - 1;                          // rows [64 cwg, 64 cwg + 64) of the tile
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  const uint32_t smem0 = smem_u32(smem);
+  int stage = 0; uint32_t phase = 0;
+  int stat_nt = -1;
+  auto flush_stats = [&](int nt_done) {
+    consumer_bar_sync();
+    const int n0s = p.n_lo + nt_done * p.TN;
+    double* o = p.stats + (int64_t)(blockIdx.x % SG_STAT_SLICES) * 2 * p.nc;
+    for (int c = ctid; c < p.TN; c += 256) {
+      atomicAdd(o + n0s + c, (double)colstat[c]);
+      atomicAdd(o + p.nc + n0s + c, (double)colstat[256 + c]);
+      colstat[c] = 0.f;
+      colstat[256 + c] = 0.f;
     }
-  } else {
-    // ================= epilogue (warps 2..9, both CTAs; each CTA owns 128 of the 256 rows) =========
-    const int quad = warp & 3;                 // TMEM lane quadrant a warp may read = warp id % 4
-    const int half = (warp - 2) >> 2;          // the two warps of a quadrant take alternate 32-column chunks
-    const int row = quad * 32 + lane;
-    int acc = 0; uint32_t acc_phase = 0;
-    const int out_buf_rows = p.out_rows + 2 * p.out_halo;
-    const int out2_buf_rows = p.out_rows + 2 * p.out2_halo;
-    // fused BatchNorm statistics (modules.py:100): per-column sum / sum of squares of the stored (rounded)
-    // outputs, accumulated per CTA in shared memory across its tiles of one N tile, flushed with one double
-    // atomic per column when the N tile changes and at the end
-    float* colstat = reinterpret_cast<float*>(smem + STAGES2 * STAGE2_BYTES + 256);
-    const int et = threadIdx.x - 64;           // 0..255 within the epilogue warps
-    int stat_nt = -1;
-    const int tb = row / p.TR, tr = row - tb * p.TR;      // this thread's (batch, row) inside an M tile: tile-invariant
-    auto flush_stats = [&](int nt_done) {
-      epi2_bar_sync();
-      const int n0s = p.n_lo + nt_done * p.TN;
-      double* o = p.stats + (int64_t)(blockIdx.x % SG_STAT_SLICES) * 2 * p.nc;
-      for (int c = et; c < p.TN; c += 256) {
-        atomicAdd(o + n0s + c, (double)colstat[c]);
-        atomicAdd(o + p.nc + n0s + c, (double)colstat[256 + c]);
-        colstat[c] = 0.f;
-        colstat[256 + c] = 0.f;
-      }
-      epi2_bar_sync();
-    };
-    if (STF && p.stats != nullptr) {
-      for (int c = et; c < 512; c += 256) colstat[c] = 0.f;
-      epi2_bar_sync();
+    consumer_bar_sync();
+  };
+  const bool tl_on = (p.dbg & (1 << 20)) && ctid == 0 && blockIdx.x < TL_CTAS;
+  int tl_i = 0;
+  unsigned long long* tl = g_tc_timeline + (blockIdx.x < TL_CTAS ? blockIdx.x : 0) * TL_SLOTS;
+  if (tl_on) { for (int i = 0; i < TL_SLOTS; ++i) tl[i] = 0; tl[tl_i++] = gtime_ns(); }
+
+  float acc[TN / 2];
+  while (it.next(p, pc)) {
+    const int ks = p.ksplit == 1 ? 0 : pc.rest % p.ksplit;
+    const int nt = p.ksplit == 1 ? pc.rest : pc.rest / p.ksplit;
+    const int n0 = p.n_lo + nt * p.TN;
+    const bool partial = pc.kb != 0 || pc.ke != pc.total;         // one K range of a split tile
+    if (p.stats != nullptr && nt != stat_nt) {
+      if (stat_nt >= 0) flush_stats(stat_nt);
+      stat_nt = nt;
     }
-    const bool tl_on = DBG && (p.dbg & (1 << 20)) && warp == 2 && lane == 0 && blockIdx.x < 160;
-    int tl_i = 0;
-    unsigned long long* tl = g_tc2_timeline + (blockIdx.x < 160 ? blockIdx.x : 0) * TL_SLOTS;
-    if (tl_on) { for (int i = 0; i < TL_SLOTS; ++i) tl[i] = 0; tl[tl_i++] = gtime_ns(); }
-    while (it.template next<SKF>(p, pc)) {
-      const int ks = (!KSF || p.ksplit == 1) ? 0 : pc.rest % p.ksplit;
-      const int nt = (!KSF || p.ksplit == 1) ? pc.rest : pc.rest / p.ksplit;
-      const int mt = 2 * pc.mp + (int)rank;
-      const int mtb = p.m_tiles_per_b == 1 ? mt : mt / p.m_tiles_per_b;
-      const int b0 = mtb * p.TB;
-      const int m0 = p.m_lo + (mt - mtb * p.m_tiles_per_b) * p.TR;
-      const int n0 = p.n_lo + nt * p.TN;
-      const int b = b0 + tb, m = m0 + tr;
-      const bool valid = (mt < m_tiles) && (tb < p.TB) && (b < p.batch) && (m < p.m_hi);
-      const bool partial = SKF && (pc.kb != 0 || pc.ke != pc.total);         // one K range of a split tile
-      if (STF && p.stats != nullptr && nt != stat_nt) {
-        if (stat_nt >= 0) flush_stats(stat_nt);
-        stat_nt = nt;
-      }
-      mbar_wait(&ctl->tmem_full[acc], acc_phase);
-      tc_fence_after();
+    const int nsteps = pc.ke - pc.kb;
+    if (nsteps == 0) {
+#pragma unroll
+      for (int j = 0; j < TN / 2; ++j) acc[j] = 0.f;
+    }
+    int prev = 0;
+    for (int i = 0; i < nsteps; ++i) {
+      mbar_wait(&ctl->full[stage], phase);
+      const uint32_t sa = smem0 + (uint32_t)stage * STAGE_BYTES;
+      mma_k64<TN, 0, 0, BF16>(acc, make_smem_desc(sa + (uint32_t)cwg * 8192u, 16, 1024),
+                        make_smem_desc(sa + A_STAGE_BYTES, 16, 1024), 2, 2, i == 0);
+      wgmma_wait<1>();                               // the MMAs of step i-1 have retired: free their stage
+      if (i > 0 && wg_leader) mbar_arrive(&ctl->empty[prev]);
+      prev = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    if (nsteps > 0 && wg_leader) mbar_arrive(&ctl->empty[prev]);
+    if (tl_on && tl_i < TL_SLOTS - 1) tl[tl_i++] = gtime_ns();
+
+    if (!partial) {
+      f_epilogue<TN>(p, acc, pc.mt, n0, ks, ctid, colstat);
       if (tl_on && tl_i < TL_SLOTS - 1) tl[tl_i++] = gtime_ns();
-      const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * p.TN);
-      const int64_t obase = ((int64_t)b * out_buf_rows + (m + p.out_halo)) * p.out_ld + (n0 - p.n_lo + p.out_col0);
-      // second (activated) output: same column geometry, its own halo; reflect mirror row of position m, if any
-      int64_t o2base = 0, o2mirror = -1;
-      if (ACF && p.out2 != nullptr) {
-        const int64_t rb = (int64_t)b * out2_buf_rows + p.out2_halo;
-        o2base = (rb + m) * p.out_ld + (n0 - p.n_lo + p.out_col0);
-        if (p.out2_halo > 0) {
-          int mm = 0;
-          bool has = false;
-          if (m >= 1 && m <= p.out2_halo) { mm = -m; has = true; }
-          else if (m >= p.out_rows - 1 - p.out2_halo && m <= p.out_rows - 2) { mm = 2 * (p.out_rows - 1) - m; has = true; }
-          if (has) o2mirror = (rb + mm) * p.out_ld + (n0 - p.n_lo + p.out_col0);
+      continue;
+    }
+    // split tile: this CTA's fp32 partial sums go to ITS workspace slot (plain stores, fragment order: only the same
+    // consumer thread of another CTA ever reads a value back); the warp that counts the tile's last contribution
+    // adds the sk_split slots up in slot order (deterministic) and finishes the tile.
+    constexpr int64_t SLOT_F2 = 128 * 256 / 2;
+    float2* myslot = reinterpret_cast<float2*>(p.sk_ws) + (int64_t)blockIdx.x * SLOT_F2 + ctid;
+#pragma unroll
+    for (int j = 0; j < TN / 4; ++j) __stcg(myslot + j * 256, make_float2(acc[2 * j], acc[2 * j + 1]));
+    if (tl_on && tl_i < TL_SLOTS - 1) tl[tl_i++] = gtime_ns();
+    const int slot = pc.tile - it.dp_end;
+    unsigned int* cnt = p.sk_cnt + slot * 8 + (ctid >> 5);
+    __threadfence();                               // this warp's partial sums are visible ...
+    __syncwarp();
+    unsigned int old = 0;
+    if ((ctid & 31) == 0) old = atomicAdd(cnt, 1u);    // ... before its contribution is counted
+    old = __shfl_sync(0xffffffffu, old, 0);
+    if (old + 1u == (unsigned int)p.sk_split) {
+      __threadfence();
+#pragma unroll
+      for (int j = 0; j < TN / 2; ++j) acc[j] = 0.f;
+      const float2* base0 = reinterpret_cast<const float2*>(p.sk_ws) + (int64_t)slot * p.sk_split * SLOT_F2 + ctid;
+      for (int sp = 0; sp < p.sk_split; ++sp) {
+#pragma unroll
+        for (int j = 0; j < TN / 4; ++j) {
+          const float2 t = __ldcg(base0 + sp * SLOT_F2 + j * 256);
+          acc[2 * j] += t.x; acc[2 * j + 1] += t.y;
         }
       }
-      // split tiles: this pair's fp32 partial sums go to ITS workspace slot (plain stores); the warp that counts the
-      // tile's last contribution adds the sk_split slots up in slot order (deterministic) and finishes the tile.
-      // Only the same (quadrant, half, lane) of another CTA ever reads a value back, so the slot layout is private:
-      // [pair][rank][warp][chunk][j4][lane] float4 -- every warp instruction moves 512 contiguous bytes
-      // (row-per-lane addressing touched 32 lines per instruction and made this path slower than the wave it removes).
-      const int ewarp = quad * 2 + half;
-      const int64_t slot_f4 = (int64_t)p.TN * 128 / 4;              // float4 per (pair, rank)
-      float4* myslot = reinterpret_cast<float4*>(p.sk_ws) + ((int64_t)pair_id * 2 + rank) * slot_f4 +
-                       (int64_t)ewarp * (p.TN / 64) * 256 + lane;
-      for (int c0 = half * 32; c0 < p.TN; c0 += 64) {
-        uint32_t r[32];
-        tmem_ld32(taddr + (uint32_t)c0, r);
-        tmem_ld_wait();
-        if (partial) {
-          float4* dst = myslot + (c0 >> 6) * 256;                   // this warp's (c0 / 64)-th chunk
-          if (!(DBG && (p.dbg & 8)))
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            __stcg(dst + j * 32, make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]),
-                                             __uint_as_float(r[4 * j + 2]), __uint_as_float(r[4 * j + 3])));
-          continue;
-        }
-        float v[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-        if (p.bias != nullptr && ks == 0) f_add_bias(p, v, n0 + c0);
-        if (valid) f_store_chunk<ACF>(p, v, obase, c0, n0 + c0, KSF && p.ksplit > 1, o2base, o2mirror);
-        if (STF && p.stats != nullptr) {                      // warp-uniform branch: the reduction is warp-collective
-          float q[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            float x = v[j];
-            // the statistics describe the tensor the next kernel reads: round like the store did
-            if (p.out_dtype == SG_F16) x = __half2float(__float2half_rn(x));
-            else if (p.out_dtype == SG_BF16) x = __bfloat162float(__float2bfloat16_rn(x));
-            x = valid ? x : 0.f;
-            v[j] = x;
-            q[j] = x * x;
-          }
-          const float sx = warp_transpose_reduce(v, lane);
-          const float sq = warp_transpose_reduce(q, lane);
-          atomicAdd(colstat + c0 + lane, sx);
-          atomicAdd(colstat + 256 + c0 + lane, sq);
-        }
-      }
-      tc_fence_before();
+      f_epilogue<TN>(p, acc, pc.mt, n0, 0, ctid, colstat);
       __syncwarp();
-      if (lane == 0) mbar_arrive_leader(&ctl->tmem_empty[acc]);      // one arrival per warp: 2 CTAs x 8 warps release it
-      if (++acc == nacc) { acc = 0; acc_phase ^= 1; }
-      if (tl_on && tl_i < TL_SLOTS - 1) tl[tl_i++] = gtime_ns();
-      if (partial && mt < m_tiles) {
-        const int slot = pc.tile - it.dp_end;
-        unsigned int* cnt = p.sk_cnt + ((((slot * 2 + (int)rank) * 4 + quad) * 2) + half);
-        __threadfence();                               // this warp's partial sums are visible ...
-        __syncwarp();
-        unsigned int old = 0;
-        if (lane == 0) old = atomicAdd(cnt, 1u);       // ... before its contribution is counted
-        old = __shfl_sync(0xffffffffu, old, 0);
-        if (old + 1u == (unsigned int)p.sk_split) {
-          __threadfence();
-          {
-            const float4* base0 = reinterpret_cast<const float4*>(p.sk_ws) +
-                                  ((int64_t)(slot * p.sk_split) * 2 + rank) * slot_f4 +
-                                  (int64_t)ewarp * (p.TN / 64) * 256 + lane;
-            for (int c0 = half * 32; c0 < p.TN; c0 += 64) {
-              float v[32];
-#pragma unroll
-              for (int j = 0; j < 32; ++j) v[j] = 0.f;
-              for (int sp = 0; sp < p.sk_split; ++sp) {
-                const float4* src = base0 + (int64_t)sp * 2 * slot_f4 + (c0 >> 6) * 256;
-                float4 t[8];
-                if (DBG && (p.dbg & 16)) {
-#pragma unroll
-                  for (int j = 0; j < 8; ++j) t[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-                } else
-#pragma unroll
-                for (int j = 0; j < 8; ++j) t[j] = __ldcg(src + j * 32);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  v[4 * j] += t[j].x; v[4 * j + 1] += t[j].y; v[4 * j + 2] += t[j].z; v[4 * j + 3] += t[j].w;
-                }
-              }
-              if (p.bias != nullptr) f_add_bias(p, v, n0 + c0);
-              if (valid) f_store_chunk<ACF>(p, v, obase, c0, n0 + c0, false, o2base, o2mirror);
-            }
-          }
-          __syncwarp();
-          if (lane == 0) *cnt = 0u;                    // ready for the next launch
-          if (tl_on && tl_i < TL_SLOTS - 1) tl[tl_i++] = gtime_ns() | (1ull << 63);      // flagged: finisher
-        }
-      }
-    }
-    if (tl_on && tl_i < TL_SLOTS) tl[tl_i++] = gtime_ns();
-    if (STF && p.stats != nullptr && stat_nt >= 0) flush_stats(stat_nt);
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_pair(tmem_base, 512);
-  }
-}
-
-// ------------------------------------------------------------------------------------------
-// form F on CTA pairs with the A tile REUSED across the taps (tapgemm_f_tc3).
-// tapgemm_f_tc2 fills (A 16 KB + B 16 KB) per CTA and k-step and its UMMAs read 48 KB of shared memory per
-// SM and k-step: 156 B/clk against the 128 B/clk port, i.e. an 82 % cap on the tensor pipe (measured:
-// 1.92 of 2.38 PFLOP/s at boost clocks).  The 9 taps of a k-block read the SAME activation rows shifted by
-// d = -4..4, so here a k-block's rows [m0 + d_lo, m0 + 127 + d_hi] (<= 136 rows, 17 KB) are staged ONCE and
-// every tap's UMMA uses a descriptor whose start address is shifted by (d - d_lo) x 128 B (the 128B-swizzle
-// phase of a non-1024-aligned start goes into the descriptor's base-offset field, make_smem_desc).  Fill
-// per k-block drops from 9 x 32 KB to 17 KB + 9 x 16 KB.  Two rings: A (per k-block) and B (per tap).
-// Requires 128-row M tiles (rows_m >= 128) and ksplit == 1.
-// ------------------------------------------------------------------------------------------
-constexpr int A3_STAGES = 3;
-constexpr int A3_STAGE_BYTES = 136 * 128;            // 17 KB = 17 x 1024: stages stay 1024 B aligned
-constexpr int B3_RING_BYTES = 10 * 128 * 128;        // weight ring: 10 stages of a 256-wide tile's half (16 KB),
-constexpr int B3_MAX_STAGES = 32;                    // 20 of a 128-wide one, 32 of a 64-wide one
-constexpr int SMEM3_BYTES = A3_STAGES * A3_STAGE_BYTES + B3_RING_BYTES + 1024 + 1024;
-constexpr int NUM_THREADS3 = 224;                    // warp 0: A producer, 1: MMA, 2..5: epilogue, 6: B producer
-
-struct SharedCtl3 {
-  uint64_t full_a[A3_STAGES];
-  uint64_t empty_a[A3_STAGES];
-  uint64_t full_b[B3_MAX_STAGES];
-  uint64_t empty_b[B3_MAX_STAGES];
-  uint64_t tmem_full[8];
-  uint64_t tmem_empty[8];
-  uint32_t tmem_base;
-};
-
-// tap `ti` contributes to (k-block kc0, N tile [n0, n0+TN))
-__device__ __forceinline__ bool f3_tap_valid(const FTcParams& p, int ti, int kc0, int n0) {
-  return !(n0 + p.TN <= p.tr.n_lo[ti] || n0 >= p.tr.n_hi[ti]) && kc0 >= p.tr.k_lo[ti] && kc0 < p.tr.k_hi[ti];
-}
-__device__ __forceinline__ uint32_t f3_tap_mask(const FTcParams& p, int kc0, int n0) {
-  uint32_t m = 0;
-  for (int d = p.d_lo; d <= p.d_hi; ++d)
-    if (f3_tap_valid(p, d + 4, kc0, n0)) m |= 1u << (d + 4);
-  return m;
-}
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NUM_THREADS3, 1)
-tapgemm_f_tc3(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
-              const __grid_constant__ CUtensorMap tmW, const FTcParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* smem_b = smem + A3_STAGES * A3_STAGE_BYTES;
-  SharedCtl3* ctl = reinterpret_cast<SharedCtl3*>(smem_b + B3_RING_BYTES);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmA0); prefetch_tmap(&tmA1); prefetch_tmap(&tmW);
-    for (int s = 0; s < A3_STAGES; ++s) { mbar_init(&ctl->full_a[s], 1); mbar_init(&ctl->empty_a[s], 1); }
-    for (int s = 0; s < B3_MAX_STAGES; ++s) { mbar_init(&ctl->full_b[s], 1); mbar_init(&ctl->empty_b[s], 1); }
-    for (int i = 0; i < 8; ++i) { mbar_init(&ctl->tmem_full[i], 1); mbar_init(&ctl->tmem_empty[i], 256); }
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc_pair(&ctl->tmem_base, 512);
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = ctl->tmem_base;
-
-  const int m_tiles = p.m_tiles_per_b * p.b_tiles;
-  const int m_pairs = (m_tiles + 1) / 2;
-  const int total_tiles = m_pairs * p.n_tiles;
-  const int npairs = gridDim.x / 2;
-  const int pair_id = blockIdx.x / 2;
-  const int half_n = p.TN / 2;
-  const int a_rows_box = 128 + (p.d_hi - p.d_lo);
-  const uint32_t a_bytes = (uint32_t)a_rows_box * 128u;
-  const uint32_t b_bytes = (uint32_t)half_n * 128u;
-  const int nacc = 512 / p.TN;
-  // weight ring depth: as many stages as fit (the ring's round trip -- commit -> empty -> TMA -> full -- is
-  // several thousand cycles, so short k-steps need many slots in flight)
-  int nb = B3_RING_BYTES / (int)b_bytes;
-  if (nb > B3_MAX_STAGES) nb = B3_MAX_STAGES;
-  if ((p.dbg >> 8) & 63) nb = min(nb, (p.dbg >> 8) & 63);        // timing experiments: cap the ring depth
-
-  if (warp == 0) {
-    // ================= A producer (both CTAs): one box per used k-block =================
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
-      for (int tile = pair_id; tile < total_tiles; tile += npairs) {
-        const int mp = tile % m_pairs;
-        const int nt = tile / m_pairs;
-        const int mt = 2 * mp + (int)rank;
-        const int b0 = mt / p.m_tiles_per_b;
-        const int m0 = p.m_lo + (mt % p.m_tiles_per_b) * 128;
-        const int n0 = p.n_lo + nt * p.TN;
-        for (int kc0 = 0; kc0 < p.kc; kc0 += 64) {
-          if (f3_tap_mask(p, kc0, n0) == 0) continue;
-          mbar_wait(&ctl->empty_a[stage], phase ^ 1);
-          if (leader) mbar_expect_tx(&ctl->full_a[stage], (p.dbg & 64) ? 0u : 2u * a_bytes);
-          const bool in0 = kc0 < p.a0_c;
-          if (!(p.dbg & 64))
-            tma_load_3d_pair(smem + stage * A3_STAGE_BYTES, in0 ? &tmA0 : &tmA1, &ctl->full_a[stage],
-                             in0 ? kc0 : kc0 - p.a0_c, m0 + p.d_lo + p.a_halo, b0);
-          if (++stage == A3_STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 6) {
-    // ================= B producer (both CTAs): this CTA's half of the weight tile, one box per tap ========
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
-      for (int tile = pair_id; tile < total_tiles; tile += npairs) {
-        const int nt = tile / m_pairs;
-        const int n0 = p.n_lo + nt * p.TN;
-        for (int kc0 = 0; kc0 < p.kc; kc0 += 64) {
-          const uint32_t mask = f3_tap_mask(p, kc0, n0);
-          for (int ti = p.d_lo + 4; ti <= p.d_hi + 4; ++ti) {
-            if (!((mask >> ti) & 1u)) continue;
-            mbar_wait(&ctl->empty_b[stage], phase ^ 1);
-            if (leader) mbar_expect_tx(&ctl->full_b[stage], (p.dbg & 32) ? 0u : 2u * b_bytes);
-            if (!(p.dbg & 32))
-              tma_load_3d_pair(smem_b + stage * b_bytes, &tmW, &ctl->full_b[stage], kc0,
-                               (ti - p.w_tap0) * p.nc + n0 + (int)rank * half_n, 0);
-            if (++stage == nb) { stage = 0; phase ^= 1; }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ================= MMA issuer (leader CTA only) =================
-    if (leader) {      // warp-uniform loop, one elected lane issues (see elect_one)
-      int sa = 0; uint32_t pa = 0;
-      int sb = 0; uint32_t pb = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      const uint32_t smem_a0 = smem_u32(smem);
-      const uint32_t smem_b0 = smem_u32(smem_b);
-      for (int tile = pair_id; tile < total_tiles; tile += npairs) {
-        const int nt = tile / m_pairs;
-        const int n0 = p.n_lo + nt * p.TN;
-        mbar_wait(&ctl->tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(acc * p.TN);
-        uint32_t accum = 0;
-        for (int kc0 = 0; kc0 < p.kc; kc0 += 64) {
-          const uint32_t mask = f3_tap_mask(p, kc0, n0);
-          if (mask == 0) continue;
-          mbar_wait(&ctl->full_a[sa], pa);
-          const uint32_t a_base = smem_a0 + (uint32_t)sa * A3_STAGE_BYTES;
-          for (int ti = p.d_lo + 4; ti <= p.d_hi + 4; ++ti) {
-            if (!((mask >> ti) & 1u)) continue;
-            mbar_wait(&ctl->full_b[sb], pb);
-            tc_fence_after();
-            // rows [d - d_lo, d - d_lo + 128) of the staged A rows: start address shifted by whole 128 B lines
-            // The swizzle pattern itself starts at the 1024 B aligned stage base (TMA wrote it), so the
-            // descriptor's base-offset field stays 0 although the start address is not 1024 B aligned
-            // (measured: base offset = (addr >> 7) & 7 gives wrong results, 0 is bit-correct).
-            uint64_t adesc = make_smem_desc(a_base + ((p.dbg & 16) ? 0u : (uint32_t)(ti - 4 - p.d_lo) * 128u), 16, 1024);
-            adesc &= ~((uint64_t)7 << 49);
-            const uint64_t bdesc = make_smem_desc(smem_b0 + (uint32_t)sb * b_bytes, 16, 1024);
-            if (elect_one()) {
-              if (!(p.dbg & 128)) {
-                umma_f16_pair(tmem_d, adesc, bdesc, p.idesc, accum);
-                umma_f16_pair(tmem_d, adesc + 2, bdesc + 2, p.idesc, 1u);
-                umma_f16_pair(tmem_d, adesc + 4, bdesc + 4, p.idesc, 1u);
-                umma_f16_pair(tmem_d, adesc + 6, bdesc + 6, p.idesc, 1u);
-              }
-              umma_commit_pair(&ctl->empty_b[sb]);       // frees the weight slot in both CTAs
-            }
-            __syncwarp();
-            accum = 1u;
-            if (++sb == nb) { sb = 0; pb ^= 1; }
-          }
-          if (elect_one()) umma_commit_pair(&ctl->empty_a[sa]);         // every tap of this k-block has been issued
-          __syncwarp();
-          if (++sa == A3_STAGES) { sa = 0; pa ^= 1; }
-        }
-        if (elect_one()) umma_commit_pair(&ctl->tmem_full[acc]);
-        __syncwarp();
-        if (++acc == nacc) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else {
-    // ================= epilogue (warps 2..5, both CTAs; each CTA owns 128 of the 256 rows) =========
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;
-    int acc = 0; uint32_t acc_phase = 0;
-    const int out_buf_rows = p.out_rows + 2 * p.out_halo;
-    for (int tile = pair_id; tile < total_tiles; tile += npairs) {
-      const int mp = tile % m_pairs;
-      const int nt = tile / m_pairs;
-      const int mt = 2 * mp + (int)rank;
-      const int b = mt / p.m_tiles_per_b;
-      const int m = p.m_lo + (mt % p.m_tiles_per_b) * 128 + row;
-      const int n0 = p.n_lo + nt * p.TN;
-      const bool valid = (mt < m_tiles) && (b < p.batch) && (m < p.m_hi);
-      mbar_wait(&ctl->tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * p.TN);
-      const int64_t obase = ((int64_t)b * out_buf_rows + (m + p.out_halo)) * p.out_ld + (n0 - p.n_lo + p.out_col0);
-      for (int c0 = 0; c0 < p.TN; c0 += 32) {
-        uint32_t r[32];
-        tmem_ld32(taddr + (uint32_t)c0, r);
-        tmem_ld_wait();
-        if (valid) {
-          float v[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-          if (p.bias != nullptr) {
-            const float* bp = p.bias + ((n0 + c0) % p.bias_mod);
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] += __ldg(bp + j);
-          }
-          if (p.out_dtype == SG_F32) {
-            float* o = reinterpret_cast<float*>(p.out) + obase + c0;
-#pragma unroll
-            for (int j = 0; j < 32; j += 4)
-              *reinterpret_cast<float4*>(o + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-          } else {
-            uint32_t pk[16];
-            if (p.out_dtype == SG_F16) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) {
-                pk[j] = pack_half2_sat(v[2 * j], v[2 * j + 1]);
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) {
-                __nv_bfloat162 h = __floats2bfloat162_rn(v[2 * j], v[2 * j + 1]);
-                pk[j] = *reinterpret_cast<uint32_t*>(&h);
-              }
-            }
-            uint4* o = reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.out) + obase + c0);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) o[j] = make_uint4(pk[4 * j], pk[4 * j + 1], pk[4 * j + 2], pk[4 * j + 3]);
-          }
-        }
-      }
-      tc_fence_before();
-      mbar_arrive_leader(&ctl->tmem_empty[acc]);
-      if (++acc == nacc) { acc = 0; acc_phase ^= 1; }
+      if ((ctid & 31) == 0) *cnt = 0u;             // ready for the next launch
+      if (tl_on && tl_i < TL_SLOTS - 1) tl[tl_i++] = gtime_ns() | (1ull << 63);      // flagged: finisher
     }
   }
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_pair(tmem_base, 512);
-  }
+  if (tl_on && tl_i < TL_SLOTS) tl[tl_i++] = gtime_ns();
+  if (p.stats != nullptr && stat_nt >= 0) flush_stats(stat_nt);
 }
 
 // ------------------------------------------------------------------------------------------
 // form W:  dWp[d+4][n][kc] += sum_{b,m} G[b,m,n] * A[b,m+d,kc]
-//   UMMA: M = 128 channels n (MN-major from G), N = TK channels kc (MN-major from A),
-//   K = 64 positions per stage (PB batches x PR rows).
+//   wgmma: M = 128 channels n (MN-major from G; 64 per consumer warpgroup), N = TK channels kc (MN-major
+//   from A), K = 64 positions per stage (PB batches x PR rows).
 // ------------------------------------------------------------------------------------------
 struct WTcParams {
   int a0_c, kc, nc, a_halo;
@@ -1227,319 +645,126 @@ struct WTcParams {
   float* dw; int dw_tap0;
   int g_rows, batch, ksplit;
   int PR, PB;                // K block = PB batches x PR rows = 64 positions
-  int TK;                    // N tile (kc), <= 256
   int n_tiles, k_tiles;      // nc/128, kc/TK
   int row_chunks, b_chunks;  // ceil(g_rows/PR), ceil(batch/PB)
-  uint32_t idesc;
   const float* out_scale;    // device scalar applied to the products before the atomic accumulation, or nullptr
 };
 
+template <int TK, bool BF16>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 tapgemm_w_tc(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CUtensorMap tmA0,
              const __grid_constant__ CUtensorMap tmA1, const WTcParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   SharedCtl* ctl = reinterpret_cast<SharedCtl*>(smem + STAGES * STAGE_BYTES);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmG); prefetch_tmap(&tmA0); prefetch_tmap(&tmA1);
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&ctl->full[s], 1); mbar_init(&ctl->empty[s], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&ctl->tmem_full[i], 1); mbar_init(&ctl->tmem_empty[i], 128); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&ctl->full[s], 1); mbar_init(&ctl->empty[s], 2); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(&ctl->tmem_base, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = ctl->tmem_base;
 
   const int ntaps = p.d_hi - p.d_lo + 1;
   const int total_tiles = ntaps * p.n_tiles * p.k_tiles * p.ksplit;
   const int pos_steps = p.row_chunks * p.b_chunks;
   const int steps_per_split = (pos_steps + p.ksplit - 1) / p.ksplit;
-  const int kboxes = p.TK / 64;
-  const uint32_t stage_tx = (uint32_t)(2 + kboxes) * 64u * 128u;
+  constexpr int KBOXES = TK / 64;
+  constexpr uint32_t STAGE_TX = (uint32_t)(2 + KBOXES) * 64u * 128u;
 
   // tile -> (d, n0, kc0, split); returns false when the (tap, n, kc) block is structurally zero
   auto decode = [&](int tile, int& d, int& n0, int& kc0, int& sp) -> bool {
     // taps fastest: the CTAs that run at the same time work on the SAME position range with
     // different taps / channel tiles, so G and the (row-shifted) A rows are shared through L2
     // instead of being streamed from HBM once per tap
-    const int ntaps_ = p.d_hi - p.d_lo + 1;
-    d = p.d_lo + tile % ntaps_; tile /= ntaps_;
+    d = p.d_lo + tile % ntaps; tile /= ntaps;
     const int kt = tile % p.k_tiles; tile /= p.k_tiles;
     const int nt = tile % p.n_tiles; tile /= p.n_tiles;
     sp = tile;
-    n0 = nt * 128; kc0 = kt * p.TK;
+    n0 = nt * 128; kc0 = kt * TK;
     const int ti = d + 4;
     if (n0 + 128 <= p.tr.n_lo[ti] || n0 >= p.tr.n_hi[ti]) return false;
-    if (kc0 + p.TK <= p.tr.k_lo[ti] || kc0 >= p.tr.k_hi[ti]) return false;
+    if (kc0 + TK <= p.tr.k_lo[ti] || kc0 >= p.tr.k_hi[ti]) return false;
     return true;
   };
 
-  if (warp == 0) {
-    // TMA producer: lane j issues box j (lanes 0,1: the two 64-channel G boxes; lanes 2..: the A boxes),
-    // so the 3..6 bulk copies of a stage leave as ONE warp instruction instead of a serial chain
-    if (lane < 2 + kboxes) {
+  if (wg == 0) {
+    // ================= TMA producer: two 64-channel G boxes + TK/64 A boxes per stage =================
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (threadIdx.x == 0) {
       int stage = 0; uint32_t phase = 0;
-      const bool is_g = lane < 2;
-      const int j = is_g ? lane : lane - 2;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         int d, n0, kc0, sp;
         if (!decode(tile, d, n0, kc0, sp)) continue;
         const int s_lo = sp * steps_per_split;
         const int s_hi = min(pos_steps, s_lo + steps_per_split);
-        // this lane's box: tensor map, channel coordinate, row shift, smem offset
-        const int kk = kc0 + 64 * j;
-        const CUtensorMap* map = is_g ? &tmG : (kk < p.a0_c ? &tmA0 : &tmA1);
-        const int c0 = is_g ? n0 + 64 * j : (kk < p.a0_c ? kk : kk - p.a0_c);
-        const int rshift = is_g ? 0 : d + p.a_halo;
-        const uint32_t off = is_g ? 8192u * j : (uint32_t)A_STAGE_BYTES + 8192u * j;
         int rc = s_lo % p.row_chunks, bc = s_lo / p.row_chunks;
         for (int s = s_lo; s < s_hi; ++s) {
           mbar_wait(&ctl->empty[stage], phase ^ 1);
-          if (lane == 0) mbar_expect_tx(&ctl->full[stage], stage_tx);
-          tma_load_3d(smem + stage * STAGE_BYTES + off, map, &ctl->full[stage], c0, rc * p.PR + rshift, bc * p.PB);
+          uint8_t* st = smem + stage * STAGE_BYTES;
+          mbar_expect_tx(&ctl->full[stage], STAGE_TX);
+          const int r = rc * p.PR, b = bc * p.PB;
+#pragma unroll
+          for (int j = 0; j < 2; ++j) tma_load_3d(st + 8192 * j, &tmG, &ctl->full[stage], n0 + 64 * j, r, b);
+#pragma unroll
+          for (int j = 0; j < KBOXES; ++j) {     // a kc tile may straddle the two sources: every box picks its map
+            const int kk = kc0 + 64 * j;
+            if (kk < p.a0_c) tma_load_3d(st + 2 * 8192 + 8192 * j, &tmA0, &ctl->full[stage], kk, r + d + p.a_halo, b);
+            else tma_load_3d(st + 2 * 8192 + 8192 * j, &tmA1, &ctl->full[stage], kk - p.a0_c, r + d + p.a_halo, b);
+          }
           if (++rc == p.row_chunks) { rc = 0; ++bc; }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    {                  // warp-uniform loop, one elected lane issues (see elect_one)
-      int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        int d, n0, kc0, sp;
-        if (!decode(tile, d, n0, kc0, sp)) continue;
-        const int s_lo = sp * steps_per_split;
-        const int s_hi = min(pos_steps, s_lo + steps_per_split);
-        if (s_lo >= s_hi) continue;
-        mbar_wait(&ctl->tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)acc * 256u;
-        uint32_t accum = 0;
-        for (int s = s_lo; s < s_hi; ++s) {
-          mbar_wait(&ctl->full[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
-          const uint32_t sb = sa + A_STAGE_BYTES;
-          // 16 positions = 16 lines of 128 B = 2048 B along K: +128 in descriptor address units
-          const uint64_t adesc = make_smem_desc(sa, 8192, 1024);
-          const uint64_t bdesc = make_smem_desc(sb, 8192, 1024);
-          if (elect_one()) {
-            umma_f16(tmem_d, adesc, bdesc, p.idesc, accum);
-            umma_f16(tmem_d, adesc + 128, bdesc + 128, p.idesc, 1u);
-            umma_f16(tmem_d, adesc + 256, bdesc + 256, p.idesc, 1u);
-            umma_f16(tmem_d, adesc + 384, bdesc + 384, p.idesc, 1u);
-            umma_commit(&ctl->empty[stage]);
-          }
-          __syncwarp();
-          accum = 1;
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        if (elect_one()) umma_commit(&ctl->tmem_full[acc]);
-        __syncwarp();
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
+    return;
+  }
+
+  // ================= consumers: warpgroup cwg owns gradient channels [n0 + 64 cwg, n0 + 64 cwg + 64) =========
+  setmaxnreg_inc<CONSUMER_REGS>();
+  const int ctid = threadIdx.x - 128;
+  const int cwg = wg - 1;
+  const int lane = ctid & 31, cw = (ctid >> 5) & 3;
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  const uint32_t smem0 = smem_u32(smem);
+  const float osc = p.out_scale ? __ldg(p.out_scale) : 1.f;
+  int stage = 0; uint32_t phase = 0;
+  float acc[TK / 2];
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    int d, n0, kc0, sp;
+    if (!decode(tile, d, n0, kc0, sp)) continue;
+    const int s_lo = sp * steps_per_split;
+    const int s_hi = min(pos_steps, s_lo + steps_per_split);
+    if (s_lo >= s_hi) continue;
+    int prev = 0;
+    for (int s = s_lo; s < s_hi; ++s) {
+      mbar_wait(&ctl->full[stage], phase);
+      const uint32_t st = smem0 + (uint32_t)stage * STAGE_BYTES;
+      // 16 positions = 16 lines of 128 B = 2048 B along K: +128 in descriptor address units
+      mma_k64<TK, 1, 1, BF16>(acc, make_smem_desc(st + (uint32_t)cwg * 8192u, 8192, 1024),
+                        make_smem_desc(st + 2 * 8192, 8192, 1024), 128, 128, s == s_lo);
+      wgmma_wait<1>();
+      if (s > s_lo && wg_leader) mbar_arrive(&ctl->empty[prev]);
+      prev = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
-  } else {
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;
-    int acc = 0; uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      int d, n0, kc0, sp;
-      if (!decode(tile, d, n0, kc0, sp)) continue;
-      const int s_lo = sp * steps_per_split;
-      const int s_hi = min(pos_steps, s_lo + steps_per_split);
-      if (s_lo >= s_hi) continue;
-      mbar_wait(&ctl->tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)acc * 256u;
-      float* o = p.dw + ((int64_t)(d + 4 - p.dw_tap0) * p.nc + n0 + row) * p.kc + kc0;
-      const int ti = d + 4;
-      const float osc = p.out_scale ? __ldg(p.out_scale) : 1.f;
-      for (int c0 = 0; c0 < p.TK; c0 += 32) {
-        uint32_t r[32];
-        tmem_ld32(taddr + (uint32_t)c0, r);
-        tmem_ld_wait();
-        // skip column blocks that are structurally zero for this tap
-        if (kc0 + c0 + 32 <= p.tr.k_lo[ti] || kc0 + c0 >= p.tr.k_hi[ti]) continue;
-        if (n0 + row < p.tr.n_lo[ti] || n0 + row >= p.tr.n_hi[ti]) continue;
-#pragma unroll
-        for (int j = 0; j < 32; j += 4)
-          red_add_v4(o + c0 + j, osc * __uint_as_float(r[j]), osc * __uint_as_float(r[j + 1]),
-                     osc * __uint_as_float(r[j + 2]), osc * __uint_as_float(r[j + 3]));
-      }
-      tc_fence_before();
-      mbar_arrive(&ctl->tmem_empty[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
+    wgmma_wait<0>();
+    if (wg_leader) mbar_arrive(&ctl->empty[prev]);
 
-// ------------------------------------------------------------------------------------------
-// form W on CTA pairs (cta_group::2): one 256 (n) x 256 (kc) block of a tap per pair.  Each CTA stages ITS 128
-// gradient channels (the M half it owns) and HALF of the activation tile (128 of the 256 kc columns; the pair's
-// UMMA reads both halves), so a k-step costs 32 KB of L2 -> shared traffic per SM instead of 48 KB for the same
-// math.  The single-CTA kernel is L2-feed bound (ncu, profiles/r2_v1_ncu_tapgemm.md: tensor pipe 77 % of active
-// cycles at 96 B/clk/SM of TMA traffic).
-// ------------------------------------------------------------------------------------------
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NUM_THREADS, 1)
-tapgemm_w_tc2(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CUtensorMap tmA0,
-              const __grid_constant__ CUtensorMap tmA1, const WTcParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  SharedCtl2* ctl = reinterpret_cast<SharedCtl2*>(smem + STAGES2 * STAGE2_BYTES);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmG); prefetch_tmap(&tmA0); prefetch_tmap(&tmA1);
-    for (int s = 0; s < STAGES2; ++s) { mbar_init(&ctl->full[s], 1); mbar_init(&ctl->empty[s], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&ctl->tmem_full[i], 1); mbar_init(&ctl->tmem_empty[i], 8); }
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc_pair(&ctl->tmem_base, 512);
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = ctl->tmem_base;
-
-  const int ntaps = p.d_hi - p.d_lo + 1;
-  const int n_tiles2 = p.nc / 256, k_tiles2 = p.kc / 256;
-  const int total_tiles = ntaps * n_tiles2 * k_tiles2 * p.ksplit;
-  const int pos_steps = p.row_chunks * p.b_chunks;
-  const int steps_per_split = (pos_steps + p.ksplit - 1) / p.ksplit;
-  const int npairs = gridDim.x / 2, pair_id = blockIdx.x / 2;
-
-  // taps fastest (see tapgemm_w_tc): concurrently running pairs share G and the row-shifted A rows through L2
-  auto decode = [&](int tile, int& d, int& n0, int& kc0, int& sp) -> bool {
-    d = p.d_lo + tile % ntaps; tile /= ntaps;
-    const int kt = tile % k_tiles2; tile /= k_tiles2;
-    const int nt = tile % n_tiles2; tile /= n_tiles2;
-    sp = tile;
-    n0 = nt * 256; kc0 = kt * 256;
     const int ti = d + 4;
-    if (n0 + 256 <= p.tr.n_lo[ti] || n0 >= p.tr.n_hi[ti]) return false;
-    if (kc0 + 256 <= p.tr.k_lo[ti] || kc0 >= p.tr.k_hi[ti]) return false;
-    return true;
-  };
-
-  if (warp == 0) {
-    // TMA producer: lanes 0,1 = this CTA's two 64-channel G boxes, lanes 2,3 = its two 64-column A boxes; all four
-    // signal the LEADER's full barrier (2 x 32 KB per stage)
-    if (lane < 4) {
-      int stage = 0; uint32_t phase = 0;
-      const bool is_g = lane < 2;
-      const int j = lane & 1;
-      for (int tile = pair_id; tile < total_tiles; tile += npairs) {
-        int d, n0, kc0, sp;
-        if (!decode(tile, d, n0, kc0, sp)) continue;
-        const int s_lo = sp * steps_per_split;
-        const int s_hi = min(pos_steps, s_lo + steps_per_split);
-        const int kk = kc0 + 128 * (int)rank + 64 * j;
-        const CUtensorMap* map = is_g ? &tmG : (kk < p.a0_c ? &tmA0 : &tmA1);
-        const int c0 = is_g ? n0 + 128 * (int)rank + 64 * j : (kk < p.a0_c ? kk : kk - p.a0_c);
-        const int rshift = is_g ? 0 : d + p.a_halo;
-        const uint32_t off = is_g ? 8192u * j : (uint32_t)A_STAGE_BYTES + 8192u * j;
-        int rc = s_lo % p.row_chunks, bc = s_lo / p.row_chunks;
-        for (int s = s_lo; s < s_hi; ++s) {
-          mbar_wait(&ctl->empty[stage], phase ^ 1);
-          if (leader && lane == 0) mbar_expect_tx(&ctl->full[stage], 2u * (uint32_t)STAGE2_BYTES);
-          tma_load_3d_pair(smem + stage * STAGE2_BYTES + off, map, &ctl->full[stage], c0, rc * p.PR + rshift,
-                           bc * p.PB);
-          if (++rc == p.row_chunks) { rc = 0; ++bc; }
-          if (++stage == STAGES2) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (leader) {
-      int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      for (int tile = pair_id; tile < total_tiles; tile += npairs) {
-        int d, n0, kc0, sp;
-        if (!decode(tile, d, n0, kc0, sp)) continue;
-        const int s_lo = sp * steps_per_split;
-        const int s_hi = min(pos_steps, s_lo + steps_per_split);
-        if (s_lo >= s_hi) continue;
-        mbar_wait(&ctl->tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)acc * 256u;
-        uint32_t accum = 0;
-        for (int s = s_lo; s < s_hi; ++s) {
-          mbar_wait(&ctl->full[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * STAGE2_BYTES);
-          const uint32_t sb = sa + A_STAGE_BYTES;
-          const uint64_t adesc = make_smem_desc(sa, 8192, 1024);
-          const uint64_t bdesc = make_smem_desc(sb, 8192, 1024);
-          if (elect_one()) {
-            umma_f16_pair(tmem_d, adesc, bdesc, p.idesc, accum);
-            umma_f16_pair(tmem_d, adesc + 128, bdesc + 128, p.idesc, 1u);
-            umma_f16_pair(tmem_d, adesc + 256, bdesc + 256, p.idesc, 1u);
-            umma_f16_pair(tmem_d, adesc + 384, bdesc + 384, p.idesc, 1u);
-            umma_commit_pair(&ctl->empty[stage]);
-          }
-          __syncwarp();
-          accum = 1;
-          if (++stage == STAGES2) { stage = 0; phase ^= 1; }
-        }
-        if (elect_one()) umma_commit_pair(&ctl->tmem_full[acc]);
-        __syncwarp();
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else {
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;
-    int acc = 0; uint32_t acc_phase = 0;
-    const float osc = p.out_scale ? __ldg(p.out_scale) : 1.f;
-    for (int tile = pair_id; tile < total_tiles; tile += npairs) {
-      int d, n0, kc0, sp;
-      if (!decode(tile, d, n0, kc0, sp)) continue;
-      const int s_lo = sp * steps_per_split;
-      const int s_hi = min(pos_steps, s_lo + steps_per_split);
-      if (s_lo >= s_hi) continue;
-      mbar_wait(&ctl->tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)acc * 256u;
-      const int n = n0 + 128 * (int)rank + row;                 // this thread's gradient channel
-      float* o = p.dw + ((int64_t)(d + 4 - p.dw_tap0) * p.nc + n) * p.kc + kc0;
-      const int ti = d + 4;
-      const bool row_live = n >= p.tr.n_lo[ti] && n < p.tr.n_hi[ti];
-      for (int c0 = 0; c0 < 256; c0 += 32) {
-        // column blocks / rows that are structurally zero for this tap are not even read
-        if (kc0 + c0 + 32 <= p.tr.k_lo[ti] || kc0 + c0 >= p.tr.k_hi[ti]) continue;
-        uint32_t r[32];
-        tmem_ld32(taddr + (uint32_t)c0, r);
-        tmem_ld_wait();
-        if (!row_live) continue;
 #pragma unroll
-        for (int j = 0; j < 32; j += 4)
-          red_add_v4(o + c0 + j, osc * __uint_as_float(r[j]), osc * __uint_as_float(r[j + 1]),
-                     osc * __uint_as_float(r[j + 2]), osc * __uint_as_float(r[j + 3]));
+    for (int h = 0; h < 2; ++h) {
+      const int n = n0 + 64 * cwg + cw * 16 + (lane >> 2) + 8 * h;      // this row's gradient channel
+      if (n < p.tr.n_lo[ti] || n >= p.tr.n_hi[ti]) continue;
+      float* o = p.dw + ((int64_t)(ti - p.dw_tap0) * p.nc + n) * p.kc + kc0 + 2 * (lane & 3);
+#pragma unroll
+      for (int j = 0; j < TK / 8; ++j) {
+        // column blocks that are structurally zero for this tap are not written
+        if (kc0 + 8 * j + 8 <= p.tr.k_lo[ti] || kc0 + 8 * j >= p.tr.k_hi[ti]) continue;
+        red_add_v2(o + 8 * j, osc * acc[4 * j + 2 * h], osc * acc[4 * j + 2 * h + 1]);
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_leader(&ctl->tmem_empty[acc]);    // 2 CTAs x 4 warps release the accumulator
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
     }
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_pair(tmem_base, 512);
   }
 }
 
@@ -1598,15 +823,15 @@ static int make_map2(CUtensorMap* m, const void* base, int dtype, int C, int64_t
   return SG_OK;
 }
 
-// split-K workspace: counters [tiles][2 CTAs][4 quadrants][2 warps] u32 (8 KB), then one partial-sum slot per CTA
-// pair [SK_MAX_PAIRS][2][128][256] fp32
-constexpr int SK_MAX_PAIRS = 96;
+// split-K workspace: counters [leftover tiles][8 consumer warps] u32 (8 KB), then one partial-sum slot per CTA
+// [SK_MAX_CTAS][128][256] fp32
+constexpr int SK_MAX_CTAS = 160;
 constexpr int64_t SK_CNT_BYTES = 8192;
-constexpr int64_t SK_WS_BYTES = SK_CNT_BYTES + (int64_t)SK_MAX_PAIRS * 2 * 128 * 256 * 4;
+constexpr int64_t SK_WS_BYTES = SK_CNT_BYTES + (int64_t)SK_MAX_CTAS * 128 * 256 * 4;
 int64_t tapgemm_f_workspace_bytes() { return SK_WS_BYTES; }
 int tapgemm_f_debug_timeline(unsigned long long* host_out, int max_words) {
-  const int n = max_words < 160 * TL_SLOTS ? max_words : 160 * TL_SLOTS;
-  if (cudaMemcpyFromSymbol(host_out, g_tc2_timeline, (size_t)n * sizeof(unsigned long long)) != cudaSuccess) return -1;
+  const int n = max_words < TL_CTAS * TL_SLOTS ? max_words : TL_CTAS * TL_SLOTS;
+  if (cudaMemcpyFromSymbol(host_out, g_tc_timeline, (size_t)n * sizeof(unsigned long long)) != cudaSuccess) return -1;
   return n;
 }
 // SEGAN_B200_STREAMK: 0 = off, n = largest split factor per leftover tile (default 16);
@@ -1615,7 +840,8 @@ int g_stream_k = [] { const char* e = getenv("SEGAN_B200_STREAMK"); return e ? a
 double g_sk_atomic_steps = [] { const char* e = getenv("SEGAN_B200_SK_ATOMIC"); return e ? atof(e) : 4.5; }();
 double g_sk_fixed_steps = [] { const char* e = getenv("SEGAN_B200_SK_FIXED"); return e ? atof(e) : 60.0; }();
 
-int g_cta_pair = 1;   // sg_set_cta_pair(): 0 single-CTA tiles, 1 cta_group::2 pairs, 2 pairs + A reuse across taps (tc3)
+// sg_set_cta_pair(): recorded for the C ABI; every setting runs the one sm_90a forward-form kernel
+int g_cta_pair = 1;
 
 static int num_sms() {
   static int n = 0;
@@ -1628,12 +854,11 @@ static int num_sms() {
   return n;
 }
 
+template <typename K>
+static int launch_persistent(K kern, int grid, const CUtensorMap& t0, const CUtensorMap& t1, const CUtensorMap& t2,
+                             const void* params, cudaStream_t st);
+
 int tapgemm_f_tc_launch(const sg_tapgemm_f* q, cudaStream_t st) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    SG_CHECK_CUDA(cudaFuncSetAttribute(tapgemm_f_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    attr_set = true;
-  }
   FTcParams p;
   p.a0_c = q->a0_c; p.kc = q->kc; p.nc = q->nc; p.a_halo = q->a_halo;
   p.d_lo = q->d_lo; p.d_hi = q->d_hi;
@@ -1651,16 +876,13 @@ int tapgemm_f_tc_launch(const sg_tapgemm_f* q, cudaStream_t st) {
   const int rows_m = q->m_hi - q->m_lo;
   const int ncols = q->n_hi - q->n_lo;
   if (rows_m >= 128) { p.TR = 128; p.TB = 1; }
-  else { p.TR = rows_m; p.TB = 128 / rows_m; if (p.TB > q->batch) p.TB = q->batch; if (p.TB > 256) p.TB = 256; }
+  else { p.TR = rows_m; p.TB = 128 / rows_m; if (p.TB > q->batch) p.TB = q->batch; }
   p.m_tiles_per_b = (rows_m + p.TR - 1) / p.TR;
   p.b_tiles = (q->batch + p.TB - 1) / p.TB;
   p.TN = (ncols % 256 == 0) ? 256 : (ncols % 128 == 0 ? 128 : 64);
   if ((q->tile_n == 64 || q->tile_n == 128 || q->tile_n == 256) && ncols % q->tile_n == 0 && q->tile_n < p.TN)
     p.TN = q->tile_n;      // narrow tiles: the caller split this launch off as the tail of a larger one
-  // (measured: 128-wide tiles to soften wave quantisation lose more to the 256-cycle issue
-  //  cadence and doubled A traffic than they gain -- 8.7 -> 10.6 ms/step -- so stay at 256)
   p.n_tiles = ncols / p.TN;
-  p.idesc = make_idesc(q->a_dtype == SG_BF16, q->w_dtype == SG_BF16, 0, 0, 128, p.TN);
   {
     static const int dbg_env = [] { const char* e = getenv("SEGAN_B200_DEBUG"); return e ? atoi(e) : 0; }();
     p.dbg = dbg_env;
@@ -1670,6 +892,7 @@ int tapgemm_f_tc_launch(const sg_tapgemm_f* q, cudaStream_t st) {
   p.out2 = q->out2; p.out2_halo = q->out2_halo; p.slope = q->slope; p.slope_mod = q->slope_mod;
   p.bias_mask = (p.bias_mod & (p.bias_mod - 1)) == 0 ? p.bias_mod - 1 : -1;
   p.slope_mask = (p.slope_mod > 0 && (p.slope_mod & (p.slope_mod - 1)) == 0) ? p.slope_mod - 1 : -1;
+  if (q->bn_stats != nullptr) SG_CHECK_ARG(p.ksplit == 1 && q->out_dtype != SG_F32 && q->n_lo == 0 && q->n_hi == q->nc);
   CUtensorMap tmA0, tmA1, tmW;
   const int a_buf_rows = q->a_rows + 2 * q->a_halo;
   int rc = make_map3(&tmA0, q->a0, q->a_dtype, q->a0_c, a_buf_rows, q->batch, p.TR, p.TB);
@@ -1679,107 +902,57 @@ int tapgemm_f_tc_launch(const sg_tapgemm_f* q, cudaStream_t st) {
   if (rc) return rc;
   rc = make_map2(&tmW, q->w, q->w_dtype, q->kc, (int64_t)(q->d_hi + 4 - q->w_tap0 + 1) * q->nc, p.TN);
   if (rc) return rc;
-  const int m_tiles_all = p.m_tiles_per_b * p.b_tiles;
-  if (q->bn_stats != nullptr) {
-    // fused BatchNorm statistics live in the CTA-pair kernel's epilogue
-    SG_CHECK_ARG(m_tiles_all >= 2 && p.ksplit == 1 && q->out_dtype != SG_F32 && q->n_lo == 0 && q->n_hi == q->nc);
-  }
-  if (g_cta_pair == 2 && m_tiles_all >= 2 && p.TR == 128 && p.TB == 1 && p.ksplit == 1 && q->d_hi - q->d_lo >= 2 &&
-      q->bn_stats == nullptr) {
-    // A tile staged once per k-block and reused by every tap (tapgemm_f_tc3)
-    static bool attr3 = false;
-    if (!attr3) {
-      SG_CHECK_CUDA(cudaFuncSetAttribute(tapgemm_f_tc3, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM3_BYTES));
-      attr3 = true;
+  const int tiles = p.m_tiles_per_b * p.b_tiles * p.n_tiles * p.ksplit;
+  int nctas = num_sms();
+  if (tiles < nctas) nctas = tiles;
+  // split-K over the last, partial wave (see PieceIter).  Cost model in k-steps of this launch's tile: leaving the
+  // leftover tiles whole costs `steps`; splitting each over S CTAs costs steps / S for the MMAs, the finisher's
+  // ordered sum of S partial tiles (g_sk_atomic_steps each for a 256-wide tile) and a fixed ~g_sk_fixed_steps of
+  // fences, counters and pipeline refill.  Short-K layers are left alone.
+  if (q->sk_ws != nullptr && g_stream_k > 1 && p.ksplit == 1 && q->bn_stats == nullptr && nctas <= SK_MAX_CTAS &&
+      tiles > nctas && tiles % nctas != 0) {
+    const int r = tiles % nctas;
+    int steps = 0;                                  // k-steps of a leftover tile (the last N tile: the longest)
+    for (int d = q->d_lo; d <= q->d_hi; ++d) steps += (q->tap_k_hi[d + 4] - q->tap_k_lo[d + 4]) / 64;
+    int best_s = 1;
+    double best = (double)steps;
+    int s_max = nctas / r < g_stream_k ? nctas / r : g_stream_k;
+    if (s_max > steps / 2) s_max = steps / 2;       // every piece keeps at least two k-steps
+    const double per_partial = g_sk_atomic_steps * 256.0 / p.TN;      // narrower tiles have shorter k-steps
+    for (int S = 2; S <= s_max; ++S) {
+      const double c = (double)steps / S + per_partial * S + g_sk_fixed_steps;
+      if (c < best) { best = c; best_s = S; }
     }
-    const int box_rows = 128 + (q->d_hi - q->d_lo);
-    rc = make_map3(&tmA0, q->a0, q->a_dtype, q->a0_c, a_buf_rows, q->batch, box_rows, 1);
-    if (rc) return rc;
-    if (q->a1) rc = make_map3(&tmA1, q->a1, q->a_dtype, q->a1_c, a_buf_rows, q->batch, box_rows, 1);
-    else tmA1 = tmA0;
-    if (rc) return rc;
-    rc = make_map3(&tmW, q->w, q->w_dtype, q->kc, (q->d_hi + 4 - q->w_tap0 + 1) * q->nc, 1, p.TN / 2, 1);
-    if (rc) return rc;
-    p.idesc = make_idesc(q->a_dtype == SG_BF16, q->w_dtype == SG_BF16, 0, 0, 256, p.TN);
-    const int pairs = ((m_tiles_all + 1) / 2) * p.n_tiles;
-    int npairs = num_sms() / 2;
-    if (pairs < npairs) npairs = pairs;
-    tapgemm_f_tc3<<<2 * npairs, NUM_THREADS3, SMEM3_BYTES, st>>>(tmA0, tmA1, tmW, p);
-    SG_CHECK_LAUNCH();
-    return SG_OK;
-  }
-  const bool fused_act = q->out2 != nullptr || q->slope != nullptr;
-  if (fused_act && !(m_tiles_all >= 2 && g_cta_pair != 2)) {
-    set_error("slope / out2 (fused PReLU) need the CTA-pair kernel (>= 2 M tiles)");
-    return SG_ERR_UNSUPPORTED;
-  }
-  if ((g_cta_pair || q->bn_stats != nullptr || fused_act) && m_tiles_all >= 2) {
-    // CTA-pair kernel: A box per CTA as before, weight box = TN/2 rows per CTA, M = 256 UMMA
-    rc = make_map3(&tmW, q->w, q->w_dtype, q->kc, (q->d_hi + 4 - q->w_tap0 + 1) * q->nc, 1, p.TN / 2, 1);
-    if (rc) return rc;
-    // the CTA-pair epilogue reads bias / slope with 16-byte loads
-    SG_CHECK_ARG(((reinterpret_cast<uintptr_t>(q->bias) | reinterpret_cast<uintptr_t>(q->slope)) & 15) == 0);
-    p.idesc = make_idesc(q->a_dtype == SG_BF16, q->w_dtype == SG_BF16, 0, 0, 256, p.TN);
-    const int pairs = ((m_tiles_all + 1) / 2) * p.n_tiles * p.ksplit;
-    int npairs = num_sms() / 2;
-    if (pairs < npairs) npairs = pairs;
-    // split-K over the last, partial wave (see PieceIter).  Cost model in k-steps of this launch's tile (measured,
-    // profiles/r2_streamk_sweep.txt): leaving the leftover tiles whole costs `steps`; splitting each over S pairs
-    // costs steps / S for the MMAs, the finisher's ordered sum of S partial tiles (g_sk_atomic_steps each for a
-    // 256-wide tile) and a fixed ~g_sk_fixed_steps of fences, counters and pipeline refill.  Short-K layers are
-    // left alone.
-    if (q->sk_ws != nullptr && g_stream_k > 1 && p.ksplit == 1 && q->bn_stats == nullptr && npairs <= SK_MAX_PAIRS &&
-        pairs > npairs && pairs % npairs != 0) {
-      const int r = pairs % npairs;
-      int steps = 0;                                  // k-steps of a leftover tile (the last N tile: the longest)
-      for (int d = q->d_lo; d <= q->d_hi; ++d) steps += (q->tap_k_hi[d + 4] - q->tap_k_lo[d + 4]) / 64;
-      int best_s = 1;
-      double best = (double)steps;
-      int s_max = npairs / r < g_stream_k ? npairs / r : g_stream_k;
-      if (s_max > steps / 2) s_max = steps / 2;       // every piece keeps at least two k-steps
-      const double per_partial = g_sk_atomic_steps * 256.0 / p.TN;      // narrower tiles have shorter k-steps
-      for (int S = 2; S <= s_max; ++S) {
-        const double c = (double)steps / S + per_partial * S + g_sk_fixed_steps;
-        if (c < best) { best = c; best_s = S; }
-      }
-      static const bool verbose = getenv("SEGAN_B200_SK_VERBOSE") != nullptr;
-      if (verbose)
-        fprintf(stderr, "tapgemm_f split-K: %d pair tiles on %d pairs, %d left over, %d k-steps, TN %d -> split %d\n",
-                pairs, npairs, r, steps, p.TN, (best_s > 1 && best < 0.92 * steps && steps >= 2 * best_s) ? best_s : 1);
-      if (best_s > 1 && best < 0.92 * steps && steps >= 2 * best_s) {
-        p.sk_dp_tiles = (pairs / npairs) * npairs;
-        p.sk_split = best_s;
-        p.sk_cnt = reinterpret_cast<unsigned int*>(q->sk_ws);
-        p.sk_ws = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(q->sk_ws) + SK_CNT_BYTES);
-      }
+    const bool split = best_s > 1 && best < 0.92 * steps && steps >= 2 * best_s;
+    static const bool verbose = getenv("SEGAN_B200_SK_VERBOSE") != nullptr;
+    if (verbose)
+      fprintf(stderr, "tapgemm_f split-K: %d tiles on %d CTAs, %d left over, %d k-steps, TN %d -> split %d\n",
+              tiles, nctas, r, steps, p.TN, split ? best_s : 1);
+    if (split) {
+      p.sk_dp_tiles = (tiles / nctas) * nctas;
+      p.sk_split = best_s;
+      p.sk_cnt = reinterpret_cast<unsigned int*>(q->sk_ws);
+      p.sk_ws = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(q->sk_ws) + SK_CNT_BYTES);
     }
-    const int need = (p.sk_split > 1 ? 1 : 0) | (p.stats != nullptr ? 2 : 0) | (fused_act ? 4 : 0) | (p.ksplit > 1 ? 8 : 0) |
-                     (p.dbg != 0 ? 15 : 0);
-    auto launch = [&](auto kern) -> int {
-      SG_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM2_BYTES));
-      kern<<<2 * npairs, NUM_THREADS2, SMEM2_BYTES, st>>>(tmA0, tmA1, tmW, p);
-      SG_CHECK_LAUNCH();
-      return SG_OK;
-    };
-    if (need & (2 | 8)) return launch(tapgemm_f_tc2<15>);
-    if (need == 0) return launch(tapgemm_f_tc2<0>);
-    if (need == 1) return launch(tapgemm_f_tc2<1>);
-    if (need == 4) return launch(tapgemm_f_tc2<4>);
-    return launch(tapgemm_f_tc2<5>);
   }
-  const int total = m_tiles_all * p.n_tiles * p.ksplit;
-  const int grid = total < num_sms() ? total : num_sms();
-  tapgemm_f_tc<<<grid, NUM_THREADS, SMEM_BYTES, st>>>(tmA0, tmA1, tmW, p);
-  SG_CHECK_LAUNCH();
+  const bool bf = q->a_dtype == SG_BF16;
+  if (p.TN == 256) return launch_persistent(bf ? tapgemm_f_tc<256, true> : tapgemm_f_tc<256, false>, nctas, tmA0, tmA1, tmW, &p, st);
+  if (p.TN == 128) return launch_persistent(bf ? tapgemm_f_tc<128, true> : tapgemm_f_tc<128, false>, nctas, tmA0, tmA1, tmW, &p, st);
+  return launch_persistent(bf ? tapgemm_f_tc<64, true> : tapgemm_f_tc<64, false>, nctas, tmA0, tmA1, tmW, &p, st);
+}
+
+template <typename K>
+static int launch_persistent(K kern, int grid, const CUtensorMap& t0, const CUtensorMap& t1, const CUtensorMap& t2,
+                             const void* params, cudaStream_t st) {
+  SG_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+  void* args[] = {const_cast<CUtensorMap*>(&t0), const_cast<CUtensorMap*>(&t1), const_cast<CUtensorMap*>(&t2),
+                  const_cast<void*>(params)};
+  SG_CHECK_CUDA(cudaLaunchKernel(reinterpret_cast<const void*>(kern), dim3(grid), dim3(NUM_THREADS), args,
+                                 (size_t)SMEM_BYTES, st));
   return SG_OK;
 }
 
 int tapgemm_w_tc_launch(const sg_tapgemm_w* q, cudaStream_t st) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    SG_CHECK_CUDA(cudaFuncSetAttribute(tapgemm_w_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    attr_set = true;
-  }
   WTcParams p;
   p.a0_c = q->a0_c; p.kc = q->kc; p.nc = q->nc; p.a_halo = q->a_halo;
   p.d_lo = q->d_lo; p.d_hi = q->d_hi;
@@ -1790,16 +963,14 @@ int tapgemm_w_tc_launch(const sg_tapgemm_w* q, cudaStream_t st) {
   p.dw = q->dw; p.dw_tap0 = q->dw_tap0; p.g_rows = q->g_rows; p.batch = q->batch;
   p.PR = q->g_rows >= 64 ? 64 : q->g_rows;
   p.PB = 64 / p.PR;
-  p.TK = q->kc >= 256 ? 256 : q->kc;
-  // a kc tile may straddle the two sources: every 64-channel box picks its own tensor map
+  const int TK = q->kc % 256 == 0 ? 256 : (q->kc % 128 == 0 ? 128 : 64);
   p.n_tiles = q->nc / 128;
-  p.k_tiles = q->kc / p.TK;
+  p.k_tiles = q->kc / TK;
   p.row_chunks = (q->g_rows + p.PR - 1) / p.PR;
   p.b_chunks = (q->batch + p.PB - 1) / p.PB;
   const int pos_steps = p.row_chunks * p.b_chunks;
   p.ksplit = q->ksplit < 1 ? 1 : q->ksplit;
   if (p.ksplit > pos_steps) p.ksplit = pos_steps;
-  p.idesc = make_idesc(q->g_dtype == SG_BF16, q->a_dtype == SG_BF16, 1, 1, 128, p.TK);
   p.out_scale = q->out_scale;
   CUtensorMap tmG, tmA0, tmA1;
   int rc = make_map3(&tmG, q->g, q->g_dtype, q->nc, q->g_rows, q->batch, p.PR, p.PB);
@@ -1810,27 +981,12 @@ int tapgemm_w_tc_launch(const sg_tapgemm_w* q, cudaStream_t st) {
   if (q->a1) rc = make_map3(&tmA1, q->a1, q->a_dtype, q->a1_c, a_buf_rows, q->batch, p.PR, p.PB);
   else tmA1 = tmA0;
   if (rc) return rc;
-  // SEGAN_B200_W_PAIR=0: single-CTA tiles only (A/B runs)
-  static const bool w_pair = [] { const char* e = getenv("SEGAN_B200_W_PAIR"); return !e || atoi(e) != 0; }();
-  if (w_pair && g_cta_pair && q->nc % 256 == 0 && q->kc % 256 == 0) {
-    static bool attr2 = false;
-    if (!attr2) {
-      SG_CHECK_CUDA(cudaFuncSetAttribute(tapgemm_w_tc2, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM2_BYTES));
-      attr2 = true;
-    }
-    p.idesc = make_idesc(q->g_dtype == SG_BF16, q->a_dtype == SG_BF16, 1, 1, 256, 256);
-    const int total2 = (q->d_hi - q->d_lo + 1) * (q->nc / 256) * (q->kc / 256) * p.ksplit;
-    int npairs = num_sms() / 2;
-    if (total2 < npairs) npairs = total2;
-    tapgemm_w_tc2<<<2 * npairs, NUM_THREADS, SMEM2_BYTES, st>>>(tmG, tmA0, tmA1, p);
-    SG_CHECK_LAUNCH();
-    return SG_OK;
-  }
   const int total = (q->d_hi - q->d_lo + 1) * p.n_tiles * p.k_tiles * p.ksplit;
   const int grid = total < num_sms() ? total : num_sms();
-  tapgemm_w_tc<<<grid, NUM_THREADS, SMEM_BYTES, st>>>(tmG, tmA0, tmA1, p);
-  SG_CHECK_LAUNCH();
-  return SG_OK;
+  const bool bf = q->g_dtype == SG_BF16;
+  if (TK == 256) return launch_persistent(bf ? tapgemm_w_tc<256, true> : tapgemm_w_tc<256, false>, grid, tmG, tmA0, tmA1, &p, st);
+  if (TK == 128) return launch_persistent(bf ? tapgemm_w_tc<128, true> : tapgemm_w_tc<128, false>, grid, tmG, tmA0, tmA1, &p, st);
+  return launch_persistent(bf ? tapgemm_w_tc<64, true> : tapgemm_w_tc<64, false>, grid, tmG, tmA0, tmA1, &p, st);
 }
 
 }  // namespace sg

@@ -325,7 +325,7 @@ extern "C" int sg_wave_deconv_bwd(const void* x0, int c0, const void* x1, int c1
 
 // ==========================================================================================
 // Tensor-core route for the waveform-end layers: a 64-channel im2col of the waveform(s) turns
-// the K = Cin*31 convs into single-tap tap-GEMMs (K = 64) on the tcgen05 kernels; the
+// the K = Cin*31 convs into single-tap tap-GEMMs (K = 64) on the wgmma kernels; the
 // transposed forms are a GEMM followed by a shift-add ("col2im").  These three kernels are the
 // HBM-bound glue around those GEMMs.
 // ==========================================================================================

@@ -1,9 +1,9 @@
-"""Host-side orchestration of the B200 kernels for the SEGAN+ Generator and Discriminator.
+"""Host-side orchestration of the H100 kernels for the SEGAN+ Generator and Discriminator.
 
 PyTorch is used for device memory (caching allocator), streams and parameter storage only; every
 FLOP of the hot path runs in libsegan_b200.so through the C ABI (segan_pytorch_b200._lib).
 
-Layer geometry follows the reference (file:line into /root/reference):
+Layer geometry follows the reference (file:line into santi-pdp/segan_pytorch):
   encoder block  = reflect-pad(14,15) -> Conv1d(k31,s4) -> [BatchNorm1d] -> PReLU   segan/models/modules.py:91-105
   decoder block  = ConvTranspose1d(k31,s4,p13)[:-1] -> PReLU | Tanh                 segan/models/modules.py:135-141
   G wiring       = 5 enc -> cat(z, h) -> 5 x (cat(h, alpha*skip), dec)              segan/models/generator.py:180-230
@@ -25,7 +25,7 @@ KW = 31
 
 
 def wave_on_tensor_cores():
-    """Waveform-end layers through im2col + tcgen05 tap-GEMMs (default) or the CUDA-core kernels."""
+    """Waveform-end layers through im2col + tensor-core tap-GEMMs (default) or the CUDA-core kernels."""
     return os.environ.get("SEGAN_B200_WAVE", "tc").lower() not in ("cuda", "ffma", "0")
 
 
@@ -128,7 +128,7 @@ def _require_cuda(*ts):
     for t in ts:
         if t is not None and not t.is_cuda:
             raise _lib.SeganB200Error(
-                "segan_pytorch_b200 runs on B200 GPUs only: got a CPU tensor (there is no CPU path; "
+                "segan_pytorch_b200 runs on H100 GPUs only: got a CPU tensor (there is no CPU path; "
                 "the CPU restatement under oracle/ is test infrastructure)")
 
 
@@ -187,20 +187,19 @@ class _Prof(object):
         return False
 
 
-NUM_SMS = 148
-# BatchNorm statistics in the conv epilogue (sg_tapgemm_f.bn_stats).  Off by default: measured in-process
-# (profiles/r1_v6_ab_bn_fusion.txt) the extra epilogue work costs what the separate 0.3 ms of bn_stats launches
-# cost -- the D conv GEMMs with short K are epilogue-bound -- so the fused path is kept tested but not used.
+NUM_SMS = 132      # H100 SXM
+# BatchNorm statistics in the conv epilogue (sg_tapgemm_f.bn_stats).  Off by default: the D conv GEMMs with short K
+# are epilogue-bound, so the extra epilogue work can cost what the separate bn_stats launches cost; the fused path is
+# kept tested but not used (not measured to pay off on H100).
 FUSE_BN_STATS = os.environ.get("SEGAN_B200_FUSE_BN_STATS", "0").lower() not in ("0", "off", "no", "false")
-# Off by default: measured per layer at batch 300 (profiles/r1_v4_layers_split.txt) the narrow-tile tail costs
-# about as much as the wave it replaces -- a tile's A-operand fill does not shrink with its width, so a
-# 64-wide tile is shared-memory-fill bound -- and only 1 of 12 shapes gained.
+# Off by default: a tile's A-operand fill does not shrink with its width, so a narrow-tile tail costs about as much
+# as the wave it replaces (not measured to pay off on H100).
 SPLIT_WAVES = os.environ.get("SEGAN_B200_WAVE_SPLIT", "0").lower() not in ("0", "off", "no", "false")
 
 
 def _f_tiling(rows_m, batch, ncols, tile_n=0):
-    """Mirror of tapgemm_f_tc_launch's tiling: (TB, m_tiles_per_b, TN, CTA-pair tiles, batch granularity of a
-    pair-aligned group)."""
+    """Tiling model of the optional wave-split planners below, in units of two 128-row M tiles ("pairs", NUM_SMS // 2
+    of them per wave): (TB, m_tiles_per_b, TN, pair tiles, batch granularity of a pair-aligned group)."""
     if rows_m >= 128:
         tb, mpb = 1, (rows_m + 127) // 128
     else:
@@ -215,8 +214,7 @@ def _f_tiling(rows_m, batch, ncols, tile_n=0):
 
 
 def _plan_f_split(rows_m, batch, ncols):
-    """Wave quantisation: batch 300 puts most layers just over a multiple of the 74 CTA pairs (300 pair
-    tiles = 4.05 waves -> 5).  Returns (B1, tail_tile_n): the launch is split into the first B1 batch
+    """Wave quantisation: batch 300 puts many layers just over a whole number of waves (e.g. 4.05 waves -> 5).  Returns (B1, tail_tile_n): the launch is split into the first B1 batch
     elements as whole waves of full-width tiles and the rest as one short wave of narrow tiles; (batch, 0)
     when splitting does not pay."""
     pairs_hw = NUM_SMS // 2
@@ -244,7 +242,7 @@ def _plan_f_split(rows_m, batch, ncols):
 
 
 # Off by default: bit-correct, but the two extra launches (tail GEMM + convert) and the tail kernel's own prologue
-# cost more than the partial wave they remove (profiles/r1_v6_splitk_tail.txt: 0-10 % slower per layer).
+# can cost more than the partial wave they remove (not measured to pay off on H100).
 SPLITK_TAIL = os.environ.get("SEGAN_B200_SPLITK_TAIL", "0").lower() not in ("0", "off", "no", "false")
 # PReLU (+ reflect halo) of the Generator's blocks in the tap-GEMM epilogue (sg_tapgemm_f.out2 / .slope)
 FUSE_ACT = os.environ.get("SEGAN_B200_FUSE_ACT", "1").lower() not in ("0", "off", "no", "false")
@@ -291,8 +289,7 @@ def sk_workspace(dev):
 
 
 def f_pair_tiles(rows_m, batch):
-    """M tiles of a form-F launch (mirror of tapgemm_f_tc_launch): the fused-activation epilogue lives in the
-    CTA-pair kernel, which needs at least two."""
+    """M tiles of a form-F launch (mirror of tapgemm_f_tc_launch); the fused-activation path is used from two on."""
     tb, mpb = _f_tiling(rows_m, batch, 64)[:2]
     return mpb * ((batch + tb - 1) // tb)
 
@@ -302,7 +299,7 @@ def run_f(a0, a1, a_rows, a_halo, a_dtype, w, w_dtype, kc, nc, taps, out, out_dt
           out_ld=0, out_col0=0, ksplit=1, backend=None, a0_c=None, a1_c=0, stats=None,
           out2=None, out2_halo=0, slope=None, slope_mod=0):
     """stats: optional [SL][2][nc] float64 tensor: BatchNorm batch statistics of the output, fused into the
-    epilogue of the tcgen05 CTA-pair kernel (see sg_tapgemm_f.bn_stats).
+    epilogue of the tensor-core kernel (see sg_tapgemm_f.bn_stats).
     slope (+ out2): PReLU fused into the epilogue -- into `out2` (with reflect halo) next to the raw `out`, or,
     without out2, into `out` itself (see sg_tapgemm_f.out2)."""
     n_hi = nc if n_hi is None else n_hi
@@ -382,7 +379,7 @@ def run_w(g, g_rows, g_dtype, a0, a1, a_rows, a_halo, a_dtype, kc, nc, taps, dw,
 def wgrad_ksplit(total_positions, n_tiles, taps=None, kc=None, nc=None, d_lo=-4, d_hi=4):
     """Position-range splits of a weight-gradient tap-GEMM.  With the tap table the number of non-empty
     (tap, n, kc) tiles is counted exactly (mirror of tapgemm_w_tc's decode()) and the split count is the
-    one that minimises waves / splits over the 148 SMs (297 tiles = 2.007 waves would run as 3); without
+    one that minimises waves / splits over the NUM_SMS SMs (265 tiles = 2.008 waves would run as 3); without
     it: about two waves."""
     steps = max(1, total_positions // 64)
     if taps is None:
@@ -453,7 +450,7 @@ SL = 8   # SG_STAT_SLICES: statistic buffers are [SL][n_stats][C]; the statistic
 # LOSS_SCALE at their source (sg_fc_tail_bwd / sg_l1_loss_bwd), every gradient tensor and the flat parameter-
 # gradient buckets carry the factor, and the optimiser kernels divide it out (their grad_scale argument).  16-bit
 # stores saturate at +-65504.  With fp16 gradients the weight-gradient tap-GEMMs read the forward activations
-# directly (same 16-bit format on both tcgen05 operands), so no bf16 twins are written.
+# directly (same 16-bit format on both wgmma operands), so no bf16 twins are written.
 # SEGAN_B200_GRAD_DTYPE=bf16 (or set_grad_dtype('bf16')) restores round 1's bf16 gradient tensors + twins
 # (loss scale 1): the measured control for the parity gates (DESIGN.md section 4).
 if os.environ.get("SEGAN_B200_GRAD_DTYPE", "f16").lower() == "bf16":     # _lib.load() applies the same variable
@@ -897,7 +894,7 @@ class GeneratorEngine(_NetEngine):
         hpb, ab, ddb, z16b = [None] * nl, [None] * nl, [None] * nl, None
         # The Generator has no norm layer between a contraction and its PReLU, so the activation (and the reflect
         # halo of the next conv) is written by the tap-GEMM epilogue next to the raw pre-activation: no separate
-        # pass over the tensor.  Needs the tcgen05 CTA-pair kernel (>= 2 M tiles), no bf16 twins, and tensors long
+        # pass over the tensor.  Needs the tensor-core backend, no bf16 twins, and tensors long
         # enough for the mirror logic; otherwise sg_act_fwd does it as before.
         eff_backend = default_backend() if self.backend is None else self.backend
         fuse_ok = FUSE_ACT and eff_backend == BACKEND_TCGEN05 and not twins
@@ -1346,7 +1343,7 @@ class DiscriminatorEngine(_NetEngine):
         a, hp, ss, mi, hpb = [None] * nl, [None] * nl, [None] * nl, [None] * nl, [None] * nl
         bnorm = not self.snorm
         stats = stat_arena(buf, "d.stats", [(SL, 2, fm[l]) for l in range(nl)], dev) if (training and bnorm) else None
-        # BatchNorm statistics in the conv epilogue (tcgen05 CTA-pair kernel; needs >= 2 M tiles: B * L/4 >= 256)
+        # BatchNorm statistics in the conv epilogue (tensor-core kernel; used with B * L/4 >= 256)
         eff_backend = default_backend() if self.backend is None else self.backend
         fuse_stats = (training and bnorm and FUSE_BN_STATS and eff_backend == BACKEND_TCGEN05 and B * Lq[-1] >= 256)
         for l in range(nl):

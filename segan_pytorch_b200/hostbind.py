@@ -1,9 +1,8 @@
 """Host-side placement for the pinned staging buffers (train.py / clean.py / bench.py).
 
-A pinned buffer lands on the NUMA node of the thread that first touches it.  On a two-socket B200 host a process
-started on the far socket stages every batch across the inter-socket link: the one-step-ahead upload of
-DevicePrefetcher then no longer hides behind the step (measured: 16.3 -> 24 ms/step end to end on such a node,
-VERDICT r1 item 8).  `bind_host_to_gpu` restricts the calling process to the CPUs that sysfs reports as local to the
+A pinned buffer lands on the NUMA node of the thread that first touches it.  On a two-socket GPU host a process
+started on the far socket stages every batch across the inter-socket link, and the one-step-ahead upload of
+DevicePrefetcher may then no longer hide behind the step.  `bind_host_to_gpu` restricts the calling process to the CPUs that sysfs reports as local to the
 GPU's PCIe root *before* those buffers are allocated; it never widens the affinity it was given and does nothing when
 the information is missing."""
 import os

@@ -195,11 +195,9 @@ def allreduce_grads(eng):
 # gradient-completion order -- on a communication stream as the backward pass produces them, so only the last,
 # small chunk is exposed; with CUDA graphs the collectives are captured into the step's single graph.
 DP_OVERLAP = os.environ.get("SEGAN_B200_DP_OVERLAP", "1").lower() not in ("0", "off", "no", "false")
-# SEGAN_B200_DP_CAPTURE=1 captures the chunked collectives INSIDE the step's single CUDA graph.  Opt-in: on 2 x B200 it
-# works and is the fastest schedule (14.88 vs 15.17 ms/step, profiles/r2_bench_2gpu_*.json), but on 4 x B200 the
-# replays following the first one hang (NCCL 2.28.9, eager collectives -- barriers -- mixed with the captured ones:
-# profiles/r2_dp_4gpu_trace.txt).  Default: three graphs with one eager all-reduce per bucket between them (the
-# schedule every N was measured with: 4 x B200 14.63 ms/step).
+# SEGAN_B200_DP_CAPTURE=1 captures the chunked collectives INSIDE the step's single CUDA graph.  Opt-in: with 4 GPUs
+# the replays following the first one were seen to hang (NCCL 2.28.9, eager collectives -- barriers -- mixed with
+# the captured ones).  Default: three graphs with one eager all-reduce per bucket between them.
 DP_CAPTURE = os.environ.get("SEGAN_B200_DP_CAPTURE", "0").lower() not in ("0", "off", "no", "false")
 
 

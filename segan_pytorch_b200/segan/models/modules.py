@@ -3,7 +3,7 @@
 The blocks own ordinary nn.Conv1d / nn.ConvTranspose1d / nn.BatchNorm1d / nn.PReLU sub-modules so
 that (i) state-dict keys are identical to the reference (SURVEY.md App. B) and (ii) construction
 consumes the torch RNG in the reference's order.  Their arithmetic is NOT run through these
-sub-modules: Generator / Discriminator drive the sm_100a kernels over whole networks
+sub-modules: Generator / Discriminator drive the sm_90a kernels over whole networks
 (segan_pytorch_b200.engine)."""
 import torch.nn as nn
 

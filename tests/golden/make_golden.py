@@ -1,8 +1,8 @@
-"""Generates tests/golden/*.npz by EXECUTING THE UNMODIFIED REFERENCE (santi-pdp/segan_pytorch,
-/root/reference) on CPU.  Runs only in the authoring container; the fixtures it writes are
-committed and are what travels to the GPU box.
+"""Generates tests/golden/*.npz by EXECUTING THE UNMODIFIED REFERENCE (santi-pdp/segan_pytorch) on CPU.
+Needs a checkout of the reference (SEGAN_REFERENCE_ROOT); the fixtures it writes are committed, so the
+test-suite itself never needs the reference.
 
-    python tests/golden/make_golden.py
+    SEGAN_REFERENCE_ROOT=/path/to/segan_pytorch python tests/golden/make_golden.py
 
 Hygiene (SURVEY.md F1 / App. D): oneDNN disabled; every conv / deconv layer is first
 self-checked fp32-vs-fp64 before anything is emitted.
@@ -49,6 +49,15 @@ def seed_all(s):
     random.seed(s)
     np.random.seed(s)
     torch.manual_seed(s)
+
+
+def arr_sha(t):
+    return hashlib.sha256(np.ascontiguousarray(np.asarray(t, dtype=np.float32)).tobytes()).hexdigest()
+
+
+def seeded_randn(seed, shape):
+    torch.manual_seed(seed)
+    return torch.randn(*[int(s) for s in shape])
 
 
 def build_reference_segan(ref, **over):
@@ -170,7 +179,10 @@ def golden_train_step(ref, out, B=4):
     with quiet():
         segan.train(opts, dloader, criterion, 100, 1e-5, 100, 10 ** 9, device="cpu")
     z = segan.G.z.detach().clone()
-    d = dict(clean=clean.numpy(), noisy=noisy.numpy(), z=z.numpy(), Genh=genh["y"].numpy(),
+    # z is stored as the seeded draw that reproduces it (tests/util.golden re-draws and checks the sha256)
+    assert torch.equal(z, seeded_randn(1234, z.shape))
+    d = dict(clean=clean.numpy(), noisy=noisy.numpy(), Genh=genh["y"].numpy(),
+             **{"z.seed": np.array(1234), "z.shape": np.array(z.shape), "z.sha256": np.array(arr_sha(z))},
              d_real_loss=np.array(losses[0]), d_fake_loss=np.array(losses[1]),
              g_adv_loss=np.array(losses[2]),
              g_l1_loss=np.array(float(100 * torch.nn.functional.l1_loss(genh["y"], clean.unsqueeze(1)))),
@@ -240,6 +252,119 @@ def golden_wsegan_generate(ref, out):
     np.savez_compressed(os.path.join(out, "wsegan_generate.npz"), **d)
 
 
+def golden_oracle_direct(ref, out):
+    """The reference's own SEGAN (seed 7): G forward (eval) and D forward (train) on seeded inputs."""
+    seed_all(7)
+    with quiet():
+        rs = ref.SEGAN(reference_opts())
+    sha_G, sha_D = sd_sha(rs.G.state_dict()), sd_sha(rs.D.state_dict())      # before D's BatchNorm stats move
+    g = torch.Generator().manual_seed(3)
+    x = 0.3 * torch.randn(2, 1, 16384, generator=g)
+    z = torch.randn(2, 1024, 16, generator=g)
+    rs.G.eval()
+    with torch.no_grad():
+        y = rs.G(x, z=z)
+    xd = 0.3 * torch.randn(3, 2, 16384, generator=g)
+    rs.D.train()
+    random.seed(5)
+    with torch.no_grad():
+        yd, _ = rs.D(xd)
+    np.savez_compressed(os.path.join(out, "reference_direct.npz"), y=y.numpy(), yd=yd.numpy(),
+                        sha_G=np.array(sha_G), sha_D=np.array(sha_D))
+
+
+SNORM_UV = ("enc_blocks.3.conv.weight_u", "enc_blocks.3.conv.weight_v", "fc.0.weight_u", "fc.3.weight_v")
+SNORM_GRADS = ("enc_blocks.2.conv.weight_orig", "fc.0.weight_orig", "fc.3.weight_orig", "enc_blocks.0.conv.bias")
+
+
+def golden_snorm_discriminator(ref, out):
+    """norm_type='snorm' Discriminator (seed 111): two training passes and one eval pass on the same input --
+    outputs, power-iteration vectors after each pass, gradients of sum(D(x)) of the training passes (sampled)."""
+    seed_all(111)
+    with quiet():
+        D = ref.Discriminator(2, [64, 128, 256, 512, 1024], 31, [4, 4, 4, 4, 4], pool_type='none', pool_slen=16,
+                              norm_type='snorm', phase_shift=5)
+    d = dict(keys=np.array(list(D.state_dict().keys())), sha_D=np.array(sd_sha(D.state_dict())))
+    g = torch.Generator().manual_seed(3)
+    x = 0.3 * torch.randn(2, 2, 16384, generator=g)
+    for i, mode in enumerate(("train", "train", "eval")):
+        D.train() if mode == "train" else D.eval()
+        random.seed(5)
+        y, _ = D(x)
+        d["y.%d" % i] = y.detach().numpy()
+        for k in SNORM_UV:
+            d["uv.%d.%s" % (i, k)] = D.state_dict()[k].numpy().copy()
+        if mode == "train":
+            D.zero_grad()
+            y.sum().backward()
+            for k in SNORM_GRADS:
+                gr = dict(D.named_parameters())[k].grad.reshape(-1)
+                idx = np.sort(np.random.RandomState(hash_str(k) % (2 ** 31)).choice(
+                    gr.numel(), size=min(4096, gr.numel()), replace=False)).astype(np.int64)
+                d["grad_idx.%d.%s" % (i, k)] = idx
+                d["grad_val.%d.%s" % (i, k)] = gr[idx].numpy()
+                d["grad_norm.%d.%s" % (i, k)] = np.array(float(gr.double().norm()))
+    np.savez_compressed(os.path.join(out, "snorm_discriminator.npz"), **d)
+
+
+def golden_sum_merge_generator(ref, out):
+    """skip_merge='sum' Generator (seed 111) with random skip alphas, eval forward on seeded inputs."""
+    seed_all(111)
+    with quiet():
+        G = ref.Generator(1, [64, 128, 256, 512, 1024], 31, [4, 4, 4, 4, 4], z_dim=1024, skip_merge='sum',
+                          skip_type='alpha', skip_init='one', bias=True)
+    d = dict(sha_G_init=np.array(sd_sha(G.state_dict())))
+    g = torch.Generator().manual_seed(4)
+    skip_keys = []
+    with torch.no_grad():
+        for k, p in G.named_parameters():
+            if k.endswith("skip_k"):
+                p.copy_(0.5 + torch.rand(p.shape, generator=g))       # alphas that matter
+                skip_keys.append(k)
+    x = 0.3 * torch.randn(2, 1, 16384, generator=g)
+    z = torch.randn(2, 1024, 16, generator=g)
+    G.eval()
+    with torch.no_grad():
+        y = G(x, z=z)
+    d.update(skip_keys=np.array(skip_keys), y=y.numpy(), sha_G=np.array(sd_sha(G.state_dict())),
+             dec1_weight_shape=np.array(G.state_dict()["dec_blocks.1.deconv.weight"].shape))
+    np.savez_compressed(os.path.join(out, "sum_merge_generator.npz"), **d)
+
+
+def golden_sedataset(ref, out):
+    """The reference's SEDataset windows of the wav set tests/test_dataset.py writes (seed 1), as sha256 of the
+    float32 window bytes."""
+    import tempfile
+    from scipy.io import wavfile
+    from tests.test_dataset import _make_wavs
+    ds = ref._ref_datasets
+
+    def fake_load(path, sr=16000):                 # the reference only uses librosa for the sample count
+        rate, w = wavfile.read(path)
+        return w.astype(np.float32) / 32768.0, rate
+    ds.librosa.load = fake_load
+
+    class SeqPool(object):                         # the detached reference module cannot be pickled for mp.Pool
+        def __init__(self, n):
+            pass
+
+        def map(self, fn, args):
+            return [fn(a) for a in args]
+    import types
+    ds.mp = types.SimpleNamespace(Pool=SeqPool)
+    with tempfile.TemporaryDirectory() as tmp:
+        cdir, ndir = _make_wavs(tmp, seed=1)
+        with quiet():
+            rds = ds.SEDataset(cdir, ndir, 0.95, cache_dir=os.path.join(tmp, "cache"), slice_size=16384, stride=0.5,
+                               slice_workers=1)
+        rows = [rds[i][:4] for i in range(len(rds))]
+    assert all(c.dtype == torch.float32 and n.dtype == torch.float32 for _, c, n, _ in rows)
+    np.savez_compressed(os.path.join(out, "sedataset_windows.npz"),
+                        names=np.array([r[0] for r in rows]), slice_idx=np.array([int(r[3]) for r in rows]),
+                        sha_clean=np.array([arr_sha(r[1].numpy()) for r in rows]),
+                        sha_noisy=np.array([arr_sha(r[2].numpy()) for r in rows]))
+
+
 def main():
     torch.set_num_threads(8)
     ref = load_reference()
@@ -252,6 +377,10 @@ def main():
     golden_generate(ref, segan, out)
     golden_train_step(ref, out, B=4)
     golden_wsegan_generate(ref, out)
+    golden_oracle_direct(ref, out)
+    golden_snorm_discriminator(ref, out)
+    golden_sum_merge_generator(ref, out)
+    golden_sedataset(ref, out)
     for f in sorted(os.listdir(out)):
         if f.endswith(".npz"):
             print(f, os.path.getsize(os.path.join(out, f)))

@@ -213,19 +213,43 @@ def test_hostbind_cpulist_and_noop_without_gpu():
         assert before is None or os.sched_getaffinity(0) == before
 
 
+def _ncu_step_csv(path):
+    """A step-level ncu CSV in the format tools/step_traffic.py's ncu command writes (banner lines, one row per
+    (launch, metric)): 60 tap-GEMM launches of 100 us / 96 MB read + 34 MB written, 60 fill launches."""
+    import csv
+    with open(path, "w", newline="") as f:
+        f.write("==PROF== Connected to process 1 (python)\n")
+        w = csv.writer(f, quoting=csv.QUOTE_ALL)
+        w.writerow(["ID", "Process ID", "Process Name", "Host Name", "Kernel Name", "Context", "Stream", "Block Size",
+                    "Grid Size", "Device", "CC", "Section Name", "Metric Name", "Metric Unit", "Metric Value"])
+        for i in range(120):
+            name = ("void sg::tapgemm_f_tc<256, false>(CUtensorMap_st, CUtensorMap_st, CUtensorMap_st, sg::FTcParams)"
+                    if i % 2 == 0 else "void at::vectorized_elementwise_kernel<4, at::FillFunctor<float>>(int)")
+            vals = (("gpu__time_duration.sum", "ns", "100,000"), ("dram__bytes_read.sum", "Mbyte", "96.00"),
+                    ("dram__bytes_write.sum", "Mbyte", "34.00")) if i % 2 == 0 else \
+                   (("gpu__time_duration.sum", "us", "5.5"), ("dram__bytes_read.sum", "byte", "0"),
+                    ("dram__bytes_write.sum", "Kbyte", "512"))
+            for m, u, v in vals:
+                w.writerow([str(i), "1", "python", "127.0.0.1", name, "1", "7", "(384, 1, 1)", "(132, 1, 1)", "0",
+                            "9.0", "Command line profiler metrics", m, u, v])
+
+
 def test_step_traffic_summary_tool_and_bench_traffic(tmp_path):
-    """tools/ncu_step_summary.py on a committed ncu CSV (per-kernel aggregation), and bench.ncu_traffic() on the
-    committed step-level capture of this round (DRAM bytes per launch of the dominant kernel)."""
+    """tools/ncu_step_summary.py on a step-level ncu CSV (per-kernel aggregation), and bench.ncu_traffic() on its
+    summary (DRAM bytes per launch of the dominant kernel)."""
     import subprocess
     import sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    out = str(tmp_path / "s")
-    r = subprocess.run([sys.executable, os.path.join(root, "tools", "ncu_step_summary.py"),
-                        os.path.join(root, "profiles", "r1_v5_launches.csv"), out], capture_output=True, text=True)
+    src, out = str(tmp_path / "launches.csv"), str(tmp_path / "s")
+    _ncu_step_csv(src)
+    r = subprocess.run([sys.executable, os.path.join(root, "tools", "ncu_step_summary.py"), src, out],
+                       capture_output=True, text=True)
     assert r.returncode == 0, r.stderr
     js = json.load(open(out + ".json"))
-    assert js["total_launches"] > 100 and "tapgemm_f_tc2" in js["kernels"] and js["kernels"]["tapgemm_f_tc2"]["ms"] > 0
+    k = "tapgemm_f_tc<256, false>"
+    assert js["total_launches"] > 100 and k in js["kernels"] and js["kernels"][k]["ms"] > 0
+    assert abs(js["kernels"][k]["ms"] - 6.0) < 1e-9 and js["kernels"][k]["dram_bytes_per_launch"] == 130e6
     sys.path.insert(0, root)
     import bench
-    t = bench.ncu_traffic()
-    assert t is not None and 1e7 < t < 1e9, t          # ~130 MB per tap-GEMM launch
+    t = bench.ncu_traffic(out + ".json")
+    assert t is not None and 1e7 < t < 1e9, t          # 130 MB per tap-GEMM launch

@@ -1,6 +1,6 @@
 """CPU tests of the wav-directory dataset (SURVEY.md 8(f)-N3): slicing / preprocessing parity with the
-reference's SEDataset (run in the authoring container, where /root/reference exists) and consistency of
-the int16 + previous-sample mode with the float mode."""
+reference's SEDataset (its windows stored as checksums in tests/golden/sedataset_windows.npz) and consistency
+of the int16 + previous-sample mode with the float mode."""
 import os
 
 import numpy as np
@@ -8,8 +8,8 @@ import pytest
 import torch
 from scipy.io import wavfile
 
-from oracle import ref_import
 from segan_pytorch_b200.segan.datasets import SEDataset, collate_fn, normalize_wave_minmax, pre_emphasize
+from tests.util import arr_sha, golden
 
 
 def _make_wavs(root, lengths=(40000, 16384, 70001, 9000), seed=0):
@@ -51,34 +51,18 @@ def test_sedataset_windows_and_pcm16_mode_agree(tmp_path):
         SEDataset(cdir, ndir, 0.95, pcm16=True, random_scale=[1, 0.5])
 
 
-@pytest.mark.skipif(not ref_import.reference_available(), reason="reference tree not present")
 def test_sedataset_matches_reference(tmp_path):
+    """Every window of the reference's SEDataset on the same files (float32 bytes, by sha256) is the window of
+    ours with the same (file, slice index)."""
     cdir, ndir = _make_wavs(str(tmp_path), seed=1)
-    ref = ref_import.load_reference()._ref_datasets
-
-    def fake_load(path, sr=16000):                 # the reference only uses librosa for the sample count
-        rate, w = wavfile.read(path)
-        return w.astype(np.float32) / 32768.0, rate
-    ref.librosa.load = fake_load
-
-    class SeqPool(object):                         # the detached reference module cannot be pickled for mp.Pool
-        def __init__(self, n):
-            pass
-
-        def map(self, fn, args):
-            return [fn(a) for a in args]
-    import types
-    ref.mp = types.SimpleNamespace(Pool=SeqPool)
-    with ref_import.quiet():
-        rds = ref.SEDataset(cdir, ndir, 0.95, cache_dir=str(tmp_path / "cache"), slice_size=16384, stride=0.5,
-                            slice_workers=1)
+    r = golden("sedataset_windows.npz")
     ours = SEDataset(cdir, ndir, 0.95, slice_size=16384, stride=0.5)
-    assert len(rds) == len(ours)
+    assert len(r["names"]) == len(ours)
     got = {(it[0], int(it[3])): it for it in (ours[i] for i in range(len(ours)))}
-    for i in range(len(rds)):
-        name, c, n, t_i = rds[i][:4]
-        mine = got[(name, int(t_i))]
-        assert torch.equal(mine[1], c) and torch.equal(mine[2], n)
+    for name, t_i, sc, sn in zip(r["names"], r["slice_idx"], r["sha_clean"], r["sha_noisy"]):
+        mine = got[(str(name), int(t_i))]
+        assert mine[1].dtype == mine[2].dtype == torch.float32
+        assert arr_sha(mine[1].numpy()) == str(sc) and arr_sha(mine[2].numpy()) == str(sn)
 
 
 def test_sedataset_short_noisy_file_is_trimmed_and_padded(tmp_path):

@@ -1,6 +1,6 @@
 """Kernel-level GPU tests: every C-ABI kernel against a plain fp32 torch evaluation of the same
-formula on the same (16-bit-rounded) operands, and the tcgen05 tap-GEMMs against the FFMA ones.
-Run on the B200 box:  python -m pytest tests -m gpu"""
+formula on the same (16-bit-rounded) operands, and the wgmma tap-GEMMs against the FFMA ones.
+Run on an H100:  python -m pytest tests -m gpu"""
 import ctypes as C
 import math
 
@@ -70,7 +70,7 @@ def _restore_cta_pair():
 @pytest.mark.parametrize("backend", [BACKEND_FFMA, BACKEND_TCGEN05, 2])
 @pytest.mark.parametrize("case", ["conv_fwd", "conv_dgrad", "deconv_fwd_cat", "deconv_dgrad", "small_rows", "fc"])
 def test_tapgemm_f(backend, case):
-    """backend 1 = tcgen05 single-CTA tiles, 2 = tcgen05 CTA pairs (cta_group::2)."""
+    """backend 1 = tensor cores with sg_set_cta_pair(0), 2 = tensor cores with sg_set_cta_pair(1)."""
     _lib.load().sg_set_cta_pair(1 if backend == 2 else 0)
     if backend == 2:
         backend = BACKEND_TCGEN05
@@ -155,8 +155,8 @@ def test_tapgemm_f(backend, case):
 
 @pytest.mark.parametrize("case", ["conv_fwd", "conv_fwd_n512", "deconv_cat", "conv_dgrad_halo", "deconv_dgrad_sub", "taps3"])
 def test_tapgemm_f_a_reuse(case):
-    """sg_set_cta_pair(2): the activation rows of a k-block are staged once (<= 136 rows) and each tap's UMMA
-    reads them through a row-shifted descriptor (tapgemm_f_tc3).  Shapes with >= 128 rows per batch element,
+    """sg_set_cta_pair(2) (the activation-reuse schedule's setting; the sm_90a kernels run one schedule for every
+    setting).  Shapes with >= 128 rows per batch element,
     a partial last M tile, an odd number of M tiles, two K sources, halo'd outputs and N sub-ranges."""
     _lib.load().sg_set_cta_pair(2)
     g = _gen(8)
@@ -217,7 +217,7 @@ def test_tapgemm_f_a_reuse(case):
 
 @pytest.mark.parametrize("case", ["conv_fwd", "small_rows_two_ntiles", "wave_single_tap"])
 def test_tapgemm_f_fused_bn_stats(case):
-    """sg_tapgemm_f.bn_stats: the CTA-pair kernel's epilogue accumulates per-column sum / sum of squares of the
+    """sg_tapgemm_f.bn_stats: the tensor-core kernel's epilogue accumulates per-column sum / sum of squares of the
     stored fp16 outputs (BatchNorm1d batch statistics) -- against the same statistics computed from the output."""
     g = _gen(9)
     d_lo, d_hi, w_tap0 = -4, 4, 0
@@ -327,7 +327,7 @@ def test_wgrad_split_plan_fills_whole_waves():
         valid = sum(1 for d in range(9) for n0 in range(0, cout, 128) for k0 in range(0, 4 * cin, tk)
                     if not (n0 + 128 <= taps[2][d] or n0 >= taps[3][d] or k0 + tk <= taps[0][d] or k0 >= taps[1][d]))
         tiles = valid * ks
-        assert tiles / float(-(-tiles // 148) * 148) >= 0.8, (l, ks, tiles)
+        assert tiles / float(-(-tiles // E.NUM_SMS) * E.NUM_SMS) >= 0.8, (l, ks, tiles)
 
 
 @pytest.mark.parametrize("backend", [BACKEND_FFMA, BACKEND_TCGEN05])
@@ -353,7 +353,7 @@ def test_tapgemm_w(backend, case):
         kc, nc = 4 * cin, cout
         taps = E.tap_ranges("conv_fwd", cin, kc, nc)
         a0 = torch.randn(B, R + 2 * halo, kc, generator=g).to(torch.float16).to(DEV)
-    elif case == "conv_wide":           # 2 x 2 blocks of 256 x 256 per tap: the CTA-pair kernel (cta_group::2)
+    elif case == "conv_wide":           # 2 x 2 blocks of 256 x 256 per tap
         B, cin, cout, R, halo = 5, 128, 512, 64, 4
         kc, nc = 4 * cin, cout
         taps = E.tap_ranges("conv_fwd", cin, kc, nc)
@@ -688,21 +688,21 @@ def test_cpu_tensor_rejected_loudly():
 
 
 # ------------------------------------------------------------------------------------------------------
-# round 2: stream-K over the last partial wave and the fused PReLU (+ reflect halo) output of the CTA-pair
+# round 2: stream-K over the last partial wave and the fused PReLU (+ reflect halo) output of the tensor-core
 # forward-form kernel
 # ------------------------------------------------------------------------------------------------------
 def _sk_case(case, g):
-    """Shapes with MORE CTA-pair tiles than the 74 pairs of a B200 and a ragged last wave."""
-    if case == "conv_fwd":          # 1024 rows x 12 batches = 96 M tiles = 48 pairs x 2 N tiles = 96 = 74 + 22
+    """Shapes with MORE tiles than the 132 CTAs of an H100 and a ragged last wave."""
+    if case == "conv_fwd":          # 1024 rows x 12 batches = 96 M tiles x 2 N tiles = 192 = 132 + 60
         B, cin, cout, R, halo = 12, 64, 512, 1024, 4
         kc, nc, kind, c = 4 * cin, cout, "conv_fwd", cin
         m_lo, m_hi, out_halo = 0, R, 0
     elif case == "deconv_fwd":      # tap-dependent N ranges: tiles of different N have different k-step counts
-        B, cin, cout, R, halo = 41, 128, 128, 256, 0       # 82 M tiles = 41 pairs x 2 N tiles = 82 = 74 + 8
+        B, cin, cout, R, halo = 41, 128, 128, 256, 0       # 82 M tiles x 2 N tiles = 164 = 132 + 32
         kc, nc, kind, c = cin, 4 * cout, "deconv_fwd", cout
         m_lo, m_hi, out_halo = 0, R, 0
-    else:                           # conv_dgrad into a halo'd view, odd M-tile count (last pair has one CTA idle)
-        B, cin, cout, R, halo = 77, 64, 128, 128, 0        # rows -4..132 = 136 -> 2 M tiles x 77 = 154 -> 77 pairs
+    else:                           # conv_dgrad into a halo'd view, two M tiles per batch element (the second one short)
+        B, cin, cout, R, halo = 77, 64, 128, 128, 0        # rows -4..132 = 136 -> 2 M tiles x 77 = 154 = 132 + 22
         kc, nc, kind, c = cout, 4 * cin, "conv_dgrad", cin
         m_lo, m_hi, out_halo = -4, R + 4, 4
     w, taps = _packed_random(kind, c, kc, nc, g, torch.float16)
@@ -712,7 +712,7 @@ def _sk_case(case, g):
 
 @pytest.mark.parametrize("case", ["conv_fwd", "deconv_fwd", "conv_dgrad"])
 def test_tapgemm_f_stream_k(case):
-    """The leftover tiles of the last wave are split along K over several CTA pairs (fp32 partial sums in per-pair
+    """The leftover tiles of the last wave are split along K over several CTAs (fp32 partial sums in per-CTA
     workspace slots, summed in slot order by the warp that counts the last contribution): same result as the
     unsplit schedule up to the fp32 summation order, counters left zeroed, bitwise repeatable."""
     g = _gen(21)
@@ -757,7 +757,7 @@ def test_tapgemm_f_fused_prelu_output(halo, inplace):
     if inplace and halo:
         pytest.skip("in-place activation has no halo")
     g = _gen(22)
-    B, cin, cout, R = 12, 64, 512, 1024            # 96 pair tiles: 22 of them take the stream-K path
+    B, cin, cout, R = 12, 64, 512, 1024            # 192 tiles on 132 CTAs: 60 of them take the stream-K path
     kc, nc = 4 * cin, cout
     w, taps = _packed_random("conv_fwd", cin, kc, nc, g, torch.float16)
     a0 = torch.randn(B, R + 8, kc, generator=g).to(torch.float16).to(DEV)

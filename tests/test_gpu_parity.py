@@ -2,7 +2,7 @@
   * against the golden vectors produced by the unmodified reference (tests/golden/*.npz)
   * against the oracle on the same seeded inputs
 north_star tolerance: 1e-3 max-abs on fp32 waveforms (written below as WAVE_TOL).
-Run on the B200 box:  python -m pytest tests -m gpu"""
+Run on an H100:  python -m pytest tests -m gpu"""
 import random
 
 import numpy as np

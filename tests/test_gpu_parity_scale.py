@@ -6,7 +6,7 @@
 Every test prints, next to the kernels' error, the error of the oracle's own operand-precision control
 (oracle.operand_precision(fp16): fp32 reference arithmetic with 16-bit operand rounding only): that is the part
 of the distance to the fp32 reference that the operand FORMAT costs, independent of any kernel.
-Run on the B200 box:  python -m pytest tests -m gpu"""
+Run on an H100:  python -m pytest tests -m gpu"""
 import random
 
 import numpy as np
@@ -24,7 +24,7 @@ WAVE_TOL = 1e-3          # north_star: max-abs on fp32 waveforms
 LOSS_RTOL = 1e-3
 LOGIT_TOL = 1e-3
 RUNSTAT_TOL = 1e-4
-# Gradients.  Measured on B200 (profiles/r2_parity_probe.txt, r2_dgrad_probe.txt): with the reference's PReLU slopes
+# Gradients (tools/parity_probe.py, tools/dgrad_probe.py take them apart): with the reference's PReLU slopes
 # (init 0: the derivative jumps from 0 to 1 at 0) every parameter gradient of a train step is 5-7 % away from the
 # fp32 oracle in relative L2 -- with bf16 AND with fp16 gradient tensors alike -- and the oracle's own operand-
 # precision control (fp32 arithmetic, fp16-rounded operands, no kernel of ours involved) is just as far, tensor by

@@ -42,8 +42,21 @@ def sd_sha(sd):
     return h.hexdigest()
 
 
+def arr_sha(a):
+    return hashlib.sha256(np.ascontiguousarray(np.asarray(a, dtype=np.float32)).tobytes()).hexdigest()
+
+
 def golden(name):
-    return np.load(os.path.join(GOLDEN, name))
+    """A fixture as a dict of arrays.  An array stored as a seeded draw (keys `<k>.seed`, `<k>.shape`,
+    `<k>.sha256`: torch.manual_seed(seed); torch.randn(shape)) is re-drawn and checked against its sha256."""
+    with np.load(os.path.join(GOLDEN, name)) as f:
+        d = {k: f[k] for k in f.files}
+    for k in [k[:-len(".seed")] for k in d if k.endswith(".seed")]:
+        torch.manual_seed(int(d[k + ".seed"]))
+        a = torch.randn(*[int(s) for s in d[k + ".shape"]]).numpy()
+        assert arr_sha(a) == str(d[k + ".sha256"]), "seeded draw %s of %s does not reproduce" % (k, name)
+        d[k] = a
+    return d
 
 
 def cpu_state(module):

@@ -1,4 +1,4 @@
-"""Launches representative SEGAN+ layer shapes of the two tcgen05 tap-GEMMs at batch 300 (for ncu /
+"""Launches representative SEGAN+ layer shapes of the two tensor-core tap-GEMMs at batch 300 (for ncu /
 timing): conv fwd enc2 (Cin 128 -> 256), deconv fwd dec1 (1024 -> 256, two K sources), conv dgrad enc3,
 wgrad enc2, wgrad dec1.  Prints CUDA-event times and TFLOP/s."""
 import os
@@ -19,12 +19,10 @@ b = lambda *s: (torch.randn(*s, device=dev) * 0.5).bfloat16()
 
 
 def timeit(name, fn, flops):
-    """COMPARE = "compare": wave split on / off;  "areuse": sg_set_cta_pair(2) (A reuse) vs (1)."""
+    """COMPARE = "compare": wave split on / off;  "splitk": split-K tail on / off;  "streamk": stream-K split factors."""
     from segan_pytorch_b200 import _lib
     lib = _lib.load()
-    if COMPARE == "areuse":
-        settings = [("areuse", lambda: lib.sg_set_cta_pair(2)), ("pair", lambda: lib.sg_set_cta_pair(1))]
-    elif COMPARE == "splitk":
+    if COMPARE == "splitk":
         settings = [("splitk", lambda: setattr(E, "SPLITK_TAIL", True)), ("plain", lambda: setattr(E, "SPLITK_TAIL", False))]
     elif COMPARE == "streamk":
         # split factor of the leftover tiles of the last wave: off, forced 2..37 (cost constant ~0), then the model
@@ -113,7 +111,7 @@ def wave0():
 
 
 def dump_timeline(name):
-    """SEGAN_B200_DEBUG bit 20: per-CTA phase stamps of the LAST tapgemm_f_tc2 launch (sg_debug_timeline)."""
+    """SEGAN_B200_DEBUG bit 20: per-CTA phase stamps of the LAST tapgemm_f_tc launch (sg_debug_timeline)."""
     import ctypes as C
     from segan_pytorch_b200 import _lib
     lib = _lib.load()
@@ -122,7 +120,7 @@ def dump_timeline(name):
     lib.sg_debug_timeline.argtypes = [C.c_void_p, C.c_int]
     n = lib.sg_debug_timeline(buf, 160 * 32)
     rows = []
-    for cta in range(148):
+    for cta in range(160):
         w = [buf[cta * 32 + i] for i in range(32)]
         w = [x for x in w if x]
         if w:

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """train.py -- drop-in for the reference entry point (train.py:14-258): same flag names and
-defaults, same seeding, writes <save_path>/train.opts, trains SEGAN+ on the B200 engine.
+defaults, same seeding, writes <save_path>/train.opts, trains SEGAN+ on the H100 engine.
 
 Additive flags only: --synthetic N (N synthetic windows instead of --clean_trainset / --noisy_trainset wav
 directories), --z_device {cpu,cuda}.
@@ -61,7 +61,7 @@ def main(opts):
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     if opts.no_cuda:
-        raise SystemExit("--no-cuda: this build is the B200 engine; use the reference for CPU training")
+        raise SystemExit("--no-cuda: this build is the H100 engine; use the reference for CPU training")
     torch.cuda.set_device(local_rank)
     device = torch.device("cuda", local_rank)
     opts.cuda = True
