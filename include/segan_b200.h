@@ -404,6 +404,25 @@ int sg_last_deconv_wgrad_fold(float* dwq /* the blocks read are cleared */, int 
                               float* dalpha, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Convolutional skip connection (GSkip skip_type='conv', generator.py:43-49): nn.Conv1d(C, C, K, stride 1,
+ * padding K//2) on the encoder's [B][L][C] pre-activation.  In the grouped view [B][L/4][4C] it is a forward-form
+ * tap-GEMM with kc = nc = 4C over the taps d = -D..D, D = (K/2 + 3) / 4 (w_tap0 = 4 - D, a_halo = 0: the zero
+ * padding is the tap-GEMM's out-of-range rows):
+ *     W'[d + D][(po, co)][(pi, ci)] = W[co][ci][4d + pi - po + K/2]   (0 where that tap is outside [0, K))
+ * K must be odd and at most 33, C a multiple of 64; anything else returns SG_ERR_INVALID.
+ *   sg_skipconv_emit       W fp32 [C][C][K] (reference layout) -> w_fwd [2D+1][4C][4C] (dtype_fwd) and/or w_dgrad,
+ *                          the data-gradient operand: per-tap transpose of W' with tap d <-> -d (dtype_dgrad).
+ *                          Either destination may be NULL; dtypes SG_F16 | SG_BF16 | SG_F32.
+ *   sg_skipconv_wgrad_fold dwq fp32 [2D+1][4C][4C], the weight-gradient tap-GEMM's result over the grouped rows ->
+ *                          dw [C][C][K] += the sum of the four copies of every tap.  Leaves all of dwq zeroed
+ *                          (the copies and the structurally zero blocks the GEMM computed alike), so it needs no
+ *                          fill before the next accumulation.
+ * ------------------------------------------------------------------------------------------ */
+int sg_skipconv_emit(const float* w, int C, int K, void* w_fwd, void* w_dgrad, int dtype_fwd, int dtype_dgrad,
+                     void* stream);
+int sg_skipconv_wgrad_fold(float* dwq, int C, int K, float* dw, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Inference tail (clean.py:72 -> model.py:156 -> se_dataset.py:119-126): de-emphasis
  * x[n] = coef*x[n-1] + y[n] per utterance as a parallel scan; and the inverse used on input.
  * ------------------------------------------------------------------------------------------ */

@@ -92,6 +92,8 @@ _SIGS = {
     "sg_stft_frames": [_vp, _i, _i, _vp, _i, _i, _vp],
     "sg_logpow_l1": [_vp, _vp, _i64, _i, _i, _i, _f, _vp, _vp, _i, _f, _vp],
     "sg_stft_frames_fold": [_vp, _i, _i, _f, _vp, _vp],
+    "sg_skipconv_emit": [_vp, _i, _i, _vp, _vp, _i, _i, _vp],
+    "sg_skipconv_wgrad_fold": [_vp, _i, _i, _vp, _vp],
 }
 EXPORTS = ["sg_abi_version", "sg_last_error", "sg_device_ok", "sg_set_cta_pair", "sg_set_ew_variant",
            "sg_set_grad_dtype", "sg_set_stream_k", "sg_tapgemm_f_workspace_bytes", "sg_debug_timeline"] + list(_SIGS)

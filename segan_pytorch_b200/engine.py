@@ -527,6 +527,60 @@ def unpack_reference(kind, m, c_out, c_in, t_len):
     return m.reshape(c_out, t_len, c_in).permute(0, 2, 1).reshape(c_out, c_in * t_len).contiguous()
 
 
+# --------------------------------------------------------------------------------------------
+# convolutional skip connection (GSkip skip_type='conv', generator.py:43-49): Conv1d(C, C, K, padding K//2) on the
+# grouped rows [B][L/4][4C] is a forward-form tap-GEMM over the taps d = -D..D (include/segan_b200.h)
+# --------------------------------------------------------------------------------------------
+def skipconv_served(k):
+    """Odd kernel widths up to 33 fit the tap-GEMMs' 9-entry tap table (D <= 4); an even width makes the
+    reference's own output one sample too long (padding K//2 on both ends), so it cannot be merged either."""
+    return isinstance(k, int) and k >= 1 and k % 2 == 1 and k <= 33
+
+
+def skipconv_geometry(c, k):
+    """(d_lo, d_hi, w_tap0, forward tap table, data-gradient tap table) of the skip conv of C = c channels.  A tap's
+    valid ranges are the bounding box of its non-zero C x C blocks (skip_conv.cu's fold kernel clears the same boxes)."""
+    p, D = k // 2, (k // 2 + 3) // 4
+    fwd = [[0] * 9, [4 * c] * 9, [0] * 9, [4 * c] * 9]
+    for d in range(-D, D + 1):
+        blocks = [(po, pi) for po in range(4) for pi in range(4) if 0 <= 4 * d + pi - po + p < k]
+        pos, pis = [b[0] for b in blocks], [b[1] for b in blocks]
+        fwd[0][d + 4], fwd[1][d + 4] = min(pis) * c, (max(pis) + 1) * c
+        fwd[2][d + 4], fwd[3][d + 4] = min(pos) * c, (max(pos) + 1) * c
+    # data gradient: tap d reads the transpose of the forward tap -d (K and N ranges swap)
+    dg = [[fwd[2][8 - i] for i in range(9)], [fwd[3][8 - i] for i in range(9)],
+          [fwd[0][8 - i] for i in range(9)], [fwd[1][8 - i] for i in range(9)]]
+    return -D, D, 4 - D, fwd, dg
+
+
+def skipconv_pack_reference(w):
+    """Conv1d weight W[C][C][K] -> forward operand W'[2D+1][4C][4C] as tensor algebra (host-side twin of
+    sg_skipconv_emit): W'[d + D][(po, co)][(pi, ci)] = W[co][ci][4d + pi - po + K//2], zero outside [0, K)."""
+    c, _, k = w.shape
+    p, D = k // 2, (k // 2 + 3) // 4
+    out = torch.zeros(2 * D + 1, 4, c, 4, c, dtype=w.dtype, device=w.device)
+    for d in range(-D, D + 1):
+        for po in range(4):
+            for pi in range(4):
+                t = 4 * d + pi - po + p
+                if 0 <= t < k:
+                    out[d + D, po, :, pi, :] = w[:, :, t]
+    return out.reshape(2 * D + 1, 4 * c, 4 * c)
+
+
+def skipconv_grouped_reference(a, wp, bias=None):
+    """The tap-GEMM the engine runs, on the host: a [B][L][C] (read as [B][L/4][4C]), wp from
+    skipconv_pack_reference; rows outside the sequence read as zero.  Returns [B][L][C]."""
+    B, L, c = a.shape
+    D = (wp.shape[0] - 1) // 2
+    ag = torch.nn.functional.pad(a.reshape(B, L // 4, 4 * c), (0, 0, D, D))
+    out = torch.zeros(B, L // 4, 4 * c, dtype=a.dtype, device=a.device)
+    for d in range(-D, D + 1):
+        out += ag[:, D + d:D + d + L // 4] @ wp[d + D].t()
+    out = out.reshape(B, L, c)
+    return out if bias is None else out + bias
+
+
 # Gradient buckets are cleared by the optimiser kernels as they read them (sg_rmsprop_step clear_grad): a step
 # needs no fill launches.  KEEP_GRADS = True (tests, inspection) leaves the gradients in place after a step; the
 # next backward then zeroes the bucket itself.
@@ -789,6 +843,10 @@ class GeneratorEngine(_NetEngine):
         self.nl = len(self.fmaps)
         self.enc_bias = m.bias
         self.sum_merge = getattr(m, "skip_merge", "concat") == "sum"
+        # skip_type='conv': the skip of encoder level l is Conv1d(C, C, K)(a[l]) (weights alpha_l.skip_k.weight /
+        # .bias, small region of the bucket) and has no alpha -- every alpha use below reads 1
+        self.conv_skip = getattr(m, "skip_type", "alpha") == "conv"
+        self.skip_kw = getattr(m, "skip_kwidth", 11)
         self.packed = {}
 
     # -- weights ----------------------------------------------------------------------------
@@ -801,7 +859,8 @@ class GeneratorEngine(_NetEngine):
         for l in range(nl - 1):
             ls.append(PackedLayer("dec_blocks.%d.deconv.weight" % l, 1, self.dec_cout(l), self.dec_cin(l), 0,
                                   "Wt%d" % l, "Wtd%d" % l,
-                                  alpha_name=("alpha_%d.skip_k" % (nl - 1 - l)) if l > 0 else None,
+                                  alpha_name=(("alpha_%d.skip_k" % (nl - 1 - l)) if l > 0 and not self.conv_skip
+                                              else None),
                                   tied=(self.sum_merge and l > 0)))
         ls += [PackedLayer("enc_blocks.%d.conv.weight" % l, 0, fm[l], fm[l - 1], 0, "Wf%d" % l, "Wdg%d" % l)
                for l in range(nl - 1, 0, -1)]
@@ -836,6 +895,17 @@ class GeneratorEngine(_NetEngine):
         wg[:, :KW] = weff
         self.packed["Wg_last"] = wg.to(GT).contiguous()
         self._mark_packed("small")
+        if self.conv_skip:
+            # skip convs: grouped 16-bit operands [2D+1][4C][4C] out of the reference-layout fp32 master
+            D = (self.skip_kw // 2 + 3) // 4
+            for l in range(self.nl - 1):
+                c = self.fmaps[l]
+                wf = self.buf.get("Wsk%d" % l, (2 * D + 1, 4 * c, 4 * c), F16, dev)
+                wd = self.buf.get("Wskd%d" % l, (2 * D + 1, 4 * c, 4 * c), GT, dev)
+                _lib.call("sg_skipconv_emit", _p(self.pview("alpha_%d.skip_k.weight" % l)), c, self.skip_kw,
+                          _p(wf), _p(wd), SG_F16, GS, _stream())
+                self.packed["Wsk%d" % l], self.packed["Wskd%d" % l] = wf, wd
+                self._mark_packed("Wsk%d" % l)
         for pl in self.layers:
             self.emit(pl, self.pview(pl.alpha_name).reshape(-1) if pl.alpha_name else None)
 
@@ -867,6 +937,12 @@ class GeneratorEngine(_NetEngine):
         """alpha of the skip merged before decoder block l (None for block 0: cat(z, h))."""
         if l == 0:
             return None
+        if self.conv_skip:                       # the skip conv's output is merged unscaled
+            c, key = self.fmaps[self.nl - 1 - l], "g.ones%d" % self.fmaps[self.nl - 1 - l]
+            ones = self.buf.t.get(key)
+            if ones is None or ones.device != self.flat.device:
+                ones = self.buf.t[key] = torch.ones(c, dtype=F32, device=self.flat.device)
+            return ones
         return self.pview("alpha_%d.skip_k" % (self.nl - 1 - l)).reshape(-1)
 
     # -- forward ----------------------------------------------------------------------------
@@ -892,6 +968,9 @@ class GeneratorEngine(_NetEngine):
         a, hp = [None] * nl, [None] * nl
         # bf16 twins (only when a backward will follow): operands of the weight-gradient tap-GEMMs
         hpb, ab, ddb, z16b = [None] * nl, [None] * nl, [None] * nl, None
+        # skip_type='conv': the skip convs' outputs (what the decoder merges instead of a[l]) and their 16-bit
+        # weight-gradient operands (bf16 twin, or the output itself with fp16 gradients)
+        sk, skb = [None] * nl, [None] * nl
         # The Generator has no norm layer between a contraction and its PReLU, so the activation (and the reflect
         # halo of the next conv) is written by the tap-GEMM epilogue next to the raw pre-activation: no separate
         # pass over the tensor.  Needs the tensor-core backend, no bf16 twins, and tensors long
@@ -940,6 +1019,8 @@ class GeneratorEngine(_NetEngine):
                           _p(hp[l]), _p(hpb[l]), _p(ab[l]), st)
             if alias:
                 hpb[l], ab[l] = hp[l], a[l]
+            if self.conv_skip and l < nl - 1:
+                sk[l], skb[l] = self._skip_conv_fwd(l, a[l], B, Lq[l], buf, twins, alias)
         # ---- z
         zc = z.shape[1]
         z16 = buf.get("g.z16", (B, Lq[-1], zc), F16, dev)
@@ -982,7 +1063,7 @@ class GeneratorEngine(_NetEngine):
             if alias:
                 ddb[l] = dd[l]
             lin *= 4
-            src0, src1 = dd[l], a[nl - 2 - l]
+            src0, src1 = dd[l], (sk if self.conv_skip else a)[nl - 2 - l]
         y = torch.empty(B, 1, L, dtype=F32, device=dev)
         blast = self.pview("dec_blocks.%d.deconv.bias" % (nl - 1))
         if wave_on_tensor_cores():
@@ -997,8 +1078,26 @@ class GeneratorEngine(_NetEngine):
                       _p(self.packed["w_last_eff"]), _p(blast), _p(y), st)
         self.packs_consumed()
         ctx = dict(x=x, B=B, L=L, Lq=Lq, a=a, hp=hp, z16=z16, ad=ad, dd=dd, y=y, hpb=hpb, ab=ab, ddb=ddb,
-                   z16b=z16b, colb=colb) if want_ctx else None
+                   z16b=z16b, colb=colb, skb=skb if self.conv_skip else ab) if want_ctx else None
         return y, ctx
+
+    def _skip_conv_fwd(self, l, a_l, B, lq, buf, twins, alias):
+        """Skip conv of encoder level l on its pre-activation a_l [B][lq][C]: one tap-GEMM over the grouped rows
+        (zero padding = rows outside the sequence).  Returns (output, weight-gradient operand of the decoder)."""
+        c, dev = self.fmaps[l], a_l.device
+        d_lo, d_hi, tap0, taps, _ = skipconv_geometry(c, self.skip_kw)
+        bias_name = "alpha_%d.skip_k.bias" % l
+        bias = self.pview(bias_name) if bias_name in self.index else None
+        outs = [(buf.get("g.sk%d" % l, (B, lq, c), F16, dev), SG_F16)]
+        if twins:                                 # bf16 gradients: a bf16 twin for the decoder's weight gradient
+            outs.append((buf.get("g.skb%d" % l, (B, lq, c), GT, dev), GS))
+        self.wait_packed("Wsk%d" % l)
+        for out, dt in outs:
+            run_f(a_l, None, lq // 4, 0, SG_F16, self.packed["Wsk%d" % l], SG_F16, 4 * c, 4 * c, taps, out, dt,
+                  lq // 4, 0, 0, lq // 4, B, bias=bias, bias_mod=c, d_lo=d_lo, d_hi=d_hi, w_tap0=tap0,
+                  backend=self.backend)
+        s = outs[0][0]
+        return s, (outs[1][0] if twins else (s if alias else None))
 
     def hidden_ncl(self, ctx, only=None):
         """`hall` of generator.py:186-227 as fp32 NCL tensors (inspection path).  only: optional set of keys."""
@@ -1048,7 +1147,9 @@ class GeneratorEngine(_NetEngine):
         lin = Lq[0]
         cin = self.dec_cin(l)
         half = cin // 2
-        g_in = buf.get("g.gin%d" % l, (B, lin, cin), GT, dev)
+        # skip_type='conv': the data gradients of the blocks with a skip are written as two tensors -- decoder half
+        # and skip half -- because the skip conv's data gradient reads its half through the contiguous grouped view
+        g_in = buf.get("g.gin%d" % l, (B, lin, half if self.conv_skip else cin), GT, dev)
         gpre = buf.get("g.gpre", (B, L), F32, dev)
         gb = self.gview("dec_blocks.%d.deconv.bias" % l)
         src0 = dd[l - 1]
@@ -1058,14 +1159,20 @@ class GeneratorEngine(_NetEngine):
             colg = buf.get("g.colg", (B, lin, 64), GT, dev)
             _lib.call("sg_wave_im2col", _p(gpre), None, 1, B, L, 0, None, 0, 13, _p(colg) if GS == SG_F16 else None,
                       _p(colg) if GS != SG_F16 else None, st)
-            run_f(colg, None, lin, 0, GS, self.packed["Wg_last"], GS, 64, cin, tap_ranges("full", 0, 64, cin),
-                  g_in, GS, lin, 0, 0, lin, B, d_lo=0, d_hi=0, w_tap0=4, backend=self.backend)
+            if self.conv_skip:
+                for dst, n0 in ((g_in, 0), (buf.get("g.gsk0", (B, lin, half), GT, dev), half)):
+                    run_f(colg, None, lin, 0, GS, self.packed["Wg_last"], GS, 64, cin, tap_ranges("full", 0, 64, cin),
+                          dst, GS, lin, 0, 0, lin, B, n_lo=n0, n_hi=n0 + half, out_ld=half, out_col0=0, d_lo=0,
+                          d_hi=0, w_tap0=4, backend=self.backend)
+            else:
+                run_f(colg, None, lin, 0, GS, self.packed["Wg_last"], GS, 64, cin, tap_ranges("full", 0, 64, cin),
+                      g_in, GS, lin, 0, 0, lin, B, d_lo=0, d_hi=0, w_tap0=4, backend=self.backend)
             # dW'[n=(s,k)][kc=(src,s',c)] over position pairs; the s == s' blocks are the gradient: folded (and
             # cleared for the next step) by sg_last_deconv_wgrad_fold into dW (alpha on the skip half) and dalpha
             dwq = buf.get("g.dwq_last", (128 * 2 * cin,), F32, dev)
-            a_train = self._param("alpha_0.skip_k").requires_grad
+            a_train = not self.conv_skip and self._param("alpha_0.skip_k").requires_grad
             with on_side(side):
-                run_w(colg, lin // 2, GS, ctx["ddb"][l - 1], ctx["ab"][0], lin // 2, 0, GS, 2 * cin, 128,
+                run_w(colg, lin // 2, GS, ctx["ddb"][l - 1], ctx["skb"][0], lin // 2, 0, GS, 2 * cin, 128,
                       tap_ranges("full", 0, 2 * cin, 128), dwq, B, d_lo=0, d_hi=0, dw_tap0=4, ksplit=74,
                       a0_c=cin, a1_c=cin, backend=self.backend)
                 gw_dst = self.gview("dec_blocks.%d.deconv.weight" % l)
@@ -1077,6 +1184,8 @@ class GeneratorEngine(_NetEngine):
                 if self.sum_merge:
                     self.gview("dec_blocks.%d.deconv.weight" % l).add_(gw_dst[:half] + gw_dst[half:])
         else:
+            if self.conv_skip:
+                raise NotImplementedError("skip_type='conv' needs the tensor-core waveform route (SEGAN_B200_WAVE=tc)")
             dweff = buf.get("g.dweff", (cin, KW), F32, dev, zero=True)
             _lib.call("sg_wave_deconv_bwd", _p(src0), half, _p(src1), half, B, lin, _p(self.packed["w_last_eff"]),
                       _p(gy), _p(ctx["y"]), _p(gpre), _p(g_in), _p(dweff), _p(gb), st)
@@ -1104,7 +1213,7 @@ class GeneratorEngine(_NetEngine):
             if l == 0:
                 s0, s1 = ctx["z16b"], ctx["hpb"][nl - 1]
             else:
-                s0, s1 = ctx["ddb"][l - 1], ctx["ab"][nl - 1 - l]
+                s0, s1 = ctx["ddb"][l - 1], ctx["skb"][nl - 1 - l]
             c0, c1 = s0.shape[-1], s1.shape[-1]
             taps = tap_ranges("deconv_fwd", cout, cin, 4 * cout)
             dwp = self.mgrad(self.by_name["dec_blocks.%d.deconv.weight" % l])     # packed gradient slot (dWeff)
@@ -1116,10 +1225,17 @@ class GeneratorEngine(_NetEngine):
                 if l == 0 and reducer is not None:
                     reducer.ready(0, launch=True)              # every decoder weight gradient has been enqueued
             # data gradient w.r.t. cat(s0, s1); block 0 only needs the encoder half (z gets no gradient)
-            g_in = buf.get("g.gin%d" % l, (B, lin, cin), GT, dev)
-            run_f(g_ad, None, lin, 0, GS, self.packed["Wtd%d" % l], GS, 4 * cout, cin,
-                  tap_ranges("deconv_dgrad", cout, 4 * cout, cin), g_in, GS, lin, 0, 0, lin, B,
-                  n_lo=(cin // 2 if l == 0 else 0), n_hi=cin, backend=self.backend)
+            if self.conv_skip and l > 0:
+                g_in = buf.get("g.gin%d" % l, (B, lin, cin // 2), GT, dev)
+                for dst, n0 in ((g_in, 0), (buf.get("g.gsk%d" % (nl - 1 - l), (B, lin, cin // 2), GT, dev), cin // 2)):
+                    run_f(g_ad, None, lin, 0, GS, self.packed["Wtd%d" % l], GS, 4 * cout, cin,
+                          tap_ranges("deconv_dgrad", cout, 4 * cout, cin), dst, GS, lin, 0, 0, lin, B,
+                          n_lo=n0, n_hi=n0 + cin // 2, out_ld=cin // 2, out_col0=0, backend=self.backend)
+            else:
+                g_in = buf.get("g.gin%d" % l, (B, lin, cin), GT, dev)
+                run_f(g_ad, None, lin, 0, GS, self.packed["Wtd%d" % l], GS, 4 * cout, cin,
+                      tap_ranges("deconv_dgrad", cout, 4 * cout, cin), g_in, GS, lin, 0, 0, lin, B,
+                      n_lo=(cin // 2 if l == 0 else 0), n_hi=cin, backend=self.backend)
             g_next = g_in
         # ---- encoder blocks nl-1 .. 0
         g_hp = None
@@ -1134,9 +1250,12 @@ class GeneratorEngine(_NetEngine):
                 _lib.call("sg_act_bwd_reduce", gh_ptr, gin0.shape[-1], 0, 0, None, None, 0, _p(a[l]), SG_F16, B, Lq[l],
                           cout, None, None, _p(slope), ACT_PRELU, _p(red), _p(g_a), st)
             else:
-                gsk = buf.t["g.gin%d" % (nl - 1 - l)]
-                gadd_ptr = C.c_void_p(gsk.data_ptr() + 2 * (gsk.shape[-1] // 2))
-                _lib.call("sg_act_bwd_reduce", _p(g_hp), cout, 16, 0, None, gadd_ptr, gsk.shape[-1], _p(a[l]), SG_F16,
+                if self.conv_skip:
+                    gadd_ptr, gadd_ld = _p(self._skip_conv_bwd(l, ctx, side)), cout
+                else:
+                    gsk = buf.t["g.gin%d" % (nl - 1 - l)]
+                    gadd_ptr, gadd_ld = C.c_void_p(gsk.data_ptr() + 2 * (gsk.shape[-1] // 2)), gsk.shape[-1]
+                _lib.call("sg_act_bwd_reduce", _p(g_hp), cout, 16, 0, None, gadd_ptr, gadd_ld, _p(a[l]), SG_F16,
                           B, Lq[l], cout, None, None, _p(slope), ACT_PRELU, _p(red), _p(g_a), st)
             _lib.call("sg_stat_grads", _p(red), cout, 3, _p(self.gview("enc_blocks.%d.act.weight" % l)),
                       _p(self.gview("enc_blocks.%d.conv.bias" % l)) if self.enc_bias else None, None, st)
@@ -1169,6 +1288,34 @@ class GeneratorEngine(_NetEngine):
         if reducer is not None:
             reducer.ready(2, launch=True)
         return self.grad
+
+    def _skip_conv_bwd(self, l, ctx, side):
+        """Backward of the skip conv of encoder level l given the gradient of its output (g.gsk<l>, [B][Lq][C]):
+        the data gradient w.r.t. a[l] is returned ([B][Lq][C], the encoder's extra pre-activation gradient); the
+        weight gradient (tap-GEMM into a workspace of the grouped layout, folded into reference layout) and the
+        bias gradient run on `side`, which serialises the levels' use of the one workspace."""
+        buf, B, lq = self.buf, ctx["B"], ctx["Lq"][l]
+        c, dev = self.fmaps[l], self.flat.device
+        D = (self.skip_kw // 2 + 3) // 4
+        d_lo, d_hi, tap0, taps, taps_dg = skipconv_geometry(c, self.skip_kw)
+        g_s = buf.t["g.gsk%d" % l]
+        g_a = buf.get("g.gask%d" % l, (B, lq, c), GT, dev)
+        run_f(g_s, None, lq // 4, 0, GS, self.packed["Wskd%d" % l], GS, 4 * c, 4 * c, taps_dg, g_a, GS, lq // 4, 0, 0,
+              lq // 4, B, d_lo=d_lo, d_hi=d_hi, w_tap0=tap0, backend=self.backend)
+        cmax = self.fmaps[self.nl - 2]
+        ws = buf.get("g.dwq_sk", ((2 * D + 1) * 16 * cmax * cmax,), F32, dev)     # left zeroed by every fold
+        dwq = ws[:(2 * D + 1) * 16 * c * c]
+        with on_side(side):
+            run_w(g_s, lq // 4, GS, ctx["ab"][l], None, lq // 4, 0, GS, 4 * c, 4 * c, taps, dwq, B, d_lo=d_lo,
+                  d_hi=d_hi, dw_tap0=tap0, ksplit=wgrad_ksplit(B * lq // 4, 0, taps, 4 * c, 4 * c, d_lo, d_hi),
+                  backend=self.backend)
+            _lib.call("sg_skipconv_wgrad_fold", _p(dwq), c, self.skip_kw,
+                      _p(self.gview("alpha_%d.skip_k.weight" % l)), _stream())
+            bias_name = "alpha_%d.skip_k.bias" % l
+            if bias_name in self.index:
+                tmp = buf.get("g.sk_tmp", (SL * cmax,), F64, dev)
+                _lib.call("sg_colsum", _p(g_s), GS, B * lq, c, c, _p(self.gview(bias_name)), 1, _p(tmp), _stream())
+        return g_a
 
 
 # ============================================================================================

@@ -11,8 +11,10 @@ from ... import engine as _engine
 
 
 class GSkip(nn.Module):
-    """Learnable per-channel skip scale (generator.py:18-78).  skip_type 'alpha' | 'constant' with merge 'concat'
-    (ckpt_segan+/train.opts) or 'sum' (generator.py:72-74) is served by the kernels."""
+    """Skip connection of one encoder level (generator.py:18-78): a learnable per-channel scale (skip_type 'alpha',
+    or 'constant' = frozen) or a stride-1 Conv1d(C, C, kwidth, padding kwidth//2) (skip_type 'conv'), with merge
+    'concat' (ckpt_segan+/train.opts) or 'sum' (generator.py:72-74).  All three are served by the kernels; the
+    conv needs an odd kwidth <= 33."""
 
     def __init__(self, skip_type, size, skip_init, skip_dropout=0, merge_mode='sum', kwidth=11, bias=True):
         super().__init__()
@@ -30,7 +32,13 @@ class GSkip(nn.Module):
             if skip_type == 'constant':
                 self.skip_k.requires_grad = False
         elif skip_type == 'conv':
-            raise NotImplementedError("skip_type='conv' is a SURVEY.md 8(f)-N4 'next' row; not built yet")
+            if not _engine.skipconv_served(kwidth):
+                raise NotImplementedError(
+                    "skip_type='conv' needs an odd skip_kwidth <= 33 (got %r): an even width makes the skip one "
+                    "sample longer than the decoder input it is merged with (padding kwidth//2 on both ends), and "
+                    "wider kernels do not fit the tap-GEMMs' 9-tap table" % (kwidth,))
+            self.skip_k = nn.Conv1d(size, size, kwidth, stride=1, padding=kwidth // 2 if kwidth > 1 else 0,
+                                    bias=bias)
         else:
             raise TypeError('Unrecognized GSkip scheme: ', skip_type)
         self.skip_type = skip_type
@@ -38,6 +46,8 @@ class GSkip(nn.Module):
             raise NotImplementedError("skip_dropout > 0 is not built yet (non-default)")
 
     def __repr__(self):
+        if self.skip_type == 'conv':
+            return super().__repr__()
         return self._get_name() + ('(Alpha(1))' if self.skip_type == 'alpha' else '(Constant(1))')
 
 
@@ -124,8 +134,11 @@ class Generator(Model):
         # ---- what the kernels serve (everything else is a "next" row, SURVEY.md 8f-N4)
         self.enc_fmaps = list(fmaps)
         self.skip_merge = skip_merge
+        self.skip_type, self.skip_kwidth = skip_type, skip_kwidth
         self._served = (ninputs == 1 and skip and not no_z and skip_merge in ('concat', 'sum')
-                        and skip_type in ('alpha', 'constant') and norm_type is None
+                        and (skip_type in ('alpha', 'constant')
+                             or (skip_type == 'conv' and _engine.skipconv_served(skip_kwidth)))
+                        and norm_type is None
                         and all(k == 31 for k in kwidth) and all(k == 31 for k in dec_kwidth)
                         and all(p == 4 for p in poolings) and all(p == 4 for p in dec_poolings)
                         and list(dec_fmaps) == fmaps[::-1][1:] + [1]
