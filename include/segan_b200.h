@@ -423,6 +423,34 @@ int sg_skipconv_emit(const float* w, int C, int K, void* w_fwd, void* w_dgrad, i
 int sg_skipconv_wgrad_fold(float* dwq, int C, int K, float* dw, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Pooled Discriminator heads (pool_type 'conv' / 'gmax' / 'gavg' / 'mlp', discriminator.py:122-146,175-192) on the last
+ * tower activation h: fp16 NLC [B][Lq][C] (no halo, no roll), C a multiple of 64, Lq <= 4096.
+ *   SG_DHEAD_CONV  a[b][t] = pool_w . h[b][t] + pool_b[0]  (pool_conv = Conv1d(C, 1, 1))   logit = fc_w[Lq] . a + fc_b
+ *   SG_DHEAD_GMAX  p[b][c] = max_t h[b][t][c]  (AdaptiveMaxPool1d(1))                      logit = fc_w[C] . p + fc_b
+ *   SG_DHEAD_GAVG  p[b][c] = mean_t h[b][t][c] (AdaptiveAvgPool1d(1))                      logit = fc_w[C] . p + fc_b
+ *   SG_DHEAD_MLP   logit[b][t] = pool_w . h[b][t] + pool_b[0]  (mlp.2 = Conv1d(C, 1, 1); h is the mlp's PReLU output):
+ *                  B * Lq logits, no fc (fc_w, fc_b, pooled, g_fc_* unused), loss and d loss / d logit over all of them
+ * sg_dhead_fwd: logit fp32 [B] ([B][Lq] for mlp); pooled fp32 = a [B][Lq] (conv, int_act['avg_conv_h']) or p [B][C]; argmax int32
+ *   [B][C] (gmax only, else may be NULL): the first t holding the maximum, where a NaN replaces the running maximum
+ *   (torch's rule: the gradient goes there).  Deterministic: no atomics.
+ * sg_dhead_bwd: the backward of  weight * mean((logit - target)^2)  fused with the loss (loss_out += it; may be
+ *   NULL), or of a given d loss / d logit (g_logit_in fp32 [B] / [B][Lq], or NULL), both multiplied by grad_scale (the loss
+ *   scale, as sg_fc_tail_bwd).  Writes every element of g_h [B][Lq][C] in the gradient dtype (sg_set_grad_dtype;
+ *   gmax: zero except at the argmax).  Parameter gradients (each may be NULL: the G step) are ADDED atomically:
+ *   g_pool_w [C], g_pool_b [1] (conv, mlp), g_fc_w [Lq | C], g_fc_b [1].
+ * ------------------------------------------------------------------------------------------ */
+#define SG_DHEAD_CONV 1
+#define SG_DHEAD_GMAX 2
+#define SG_DHEAD_GAVG 3
+#define SG_DHEAD_MLP 4
+int sg_dhead_fwd(int pool_type, const void* h, int batch, int Lq, int C, const float* pool_w, const float* pool_b,
+                 const float* fc_w, const float* fc_b, float* pooled, int32_t* argmax, float* logit, void* stream);
+int sg_dhead_bwd(int pool_type, const void* h, int batch, int Lq, int C, const float* pool_w, const float* fc_w,
+                 const float* pooled, const int32_t* argmax, const float* logit, const float* g_logit_in,
+                 float target, float weight, float* loss_out, void* g_h, float* g_pool_w, float* g_pool_b,
+                 float* g_fc_w, float* g_fc_b, float grad_scale, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Inference tail (clean.py:72 -> model.py:156 -> se_dataset.py:119-126): de-emphasis
  * x[n] = coef*x[n-1] + y[n] per utterance as a parallel scan; and the inverse used on input.
  * ------------------------------------------------------------------------------------------ */

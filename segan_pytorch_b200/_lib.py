@@ -14,6 +14,7 @@ ACT_NONE, ACT_PRELU, ACT_TANH = 0, 1, 2
 EW_ACT_FWD, EW_BN_STATS, EW_BWD_REDUCE, EW_BWD_APPLY = 1, 2, 3, 4
 PCM_NO_PREV = 0x7fffffff
 BACKEND_FFMA, BACKEND_TCGEN05 = 0, 1
+SG_DHEAD_CONV, SG_DHEAD_GMAX, SG_DHEAD_GAVG, SG_DHEAD_MLP = 1, 2, 3, 4
 
 _vp, _i, _f, _i64 = C.c_void_p, C.c_int, C.c_float, C.c_int64
 I9 = C.c_int32 * 9
@@ -94,6 +95,8 @@ _SIGS = {
     "sg_stft_frames_fold": [_vp, _i, _i, _f, _vp, _vp],
     "sg_skipconv_emit": [_vp, _i, _i, _vp, _vp, _i, _i, _vp],
     "sg_skipconv_wgrad_fold": [_vp, _i, _i, _vp, _vp],
+    "sg_dhead_fwd": [_i, _vp, _i, _i, _i] + [_vp] * 8,
+    "sg_dhead_bwd": [_i, _vp, _i, _i, _i] + [_vp] * 6 + [_f, _f, _vp, _vp] + [_vp] * 4 + [_f, _vp],
 }
 EXPORTS = ["sg_abi_version", "sg_last_error", "sg_device_ok", "sg_set_cta_pair", "sg_set_ew_variant",
            "sg_set_grad_dtype", "sg_set_stream_k", "sg_tapgemm_f_workspace_bytes", "sg_debug_timeline"] + list(_SIGS)

@@ -8,7 +8,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libsegan_b200.so")
 SOURCES = ["api.cu", "tapgemm_ref.cu", "tapgemm_tc.cu", "wave_layers.cu", "elementwise.cu", "stream_ew.cu", "optim_pack.cu", "snorm.cu", "stft.cu",
-           "skip_conv.cu"]
+           "skip_conv.cu", "dhead.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 

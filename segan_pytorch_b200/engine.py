@@ -18,10 +18,12 @@ import os
 import torch
 
 from . import _lib
-from ._lib import (ACT_NONE, ACT_PRELU, BACKEND_FFMA, BACKEND_TCGEN05, SG_BF16, SG_F16, SG_F32,
-                   TapGemmF, TapGemmW)
+from ._lib import (ACT_NONE, ACT_PRELU, BACKEND_FFMA, BACKEND_TCGEN05, SG_BF16, SG_DHEAD_CONV, SG_DHEAD_GAVG,
+                   SG_DHEAD_GMAX, SG_DHEAD_MLP, SG_F16, SG_F32, TapGemmF, TapGemmW)
 
 KW = 31
+# Discriminator pool_type -> head kernel selector of sg_dhead_fwd / _bwd ('none' runs fc.0 + sg_fc_tail instead)
+DHEAD_KINDS = {"conv": SG_DHEAD_CONV, "gmax": SG_DHEAD_GMAX, "gavg": SG_DHEAD_GAVG, "mlp": SG_DHEAD_MLP}
 
 
 def wave_on_tensor_cores():
@@ -1341,22 +1343,34 @@ class DiscriminatorEngine(_NetEngine):
         # concurrently with another pass of the same network.  Both lanes accumulate into the SAME gradient
         # bucket: every parameter-gradient writer is atomic (red.add in the wgrad epilogue, atomicAdd elsewhere).
         self.buf1 = _Buffers()
+        # pool_type 'none': fc.0 (a tap-GEMM) + sg_fc_tail; 'conv' / 'gmax' / 'gavg': the small pooled heads of
+        # discriminator.py:122-137, one sg_dhead_fwd / _bwd launch each; 'mlp' (discriminator.py:138-143): its
+        # C x C 1x1 conv mlp.0 is a single-tap tap-GEMM over the B * Lq positions, the PReLU(C) mlp.1 runs on the
+        # tower's activation kernels and the per-position C -> 1 conv mlp.2 + loss on sg_dhead_fwd / _bwd
+        self.pool_type = getattr(module, "pool_type", "none")
 
     def packed_layers(self):
-        """Bucket order = gradient completion order of a backward pass: fc.0, enc4 | enc3 .. enc1, small."""
+        """Bucket order = gradient completion order of a backward pass: [fc.0 | mlp.0,] enc4 | enc3 .. enc1, small."""
         fm = self.fmaps
-        nout, kin = self._param("fc.0.weight" + self.wsfx).shape
-        ls = [PackedLayer("fc.0.weight" + self.wsfx, 2, nout, fm[-1], kin // fm[-1], "W1p", "W1dg")]
+        ls = []
+        if self.pool_type == "none":
+            nout, kin = self._param("fc.0.weight" + self.wsfx).shape
+            ls.append(PackedLayer("fc.0.weight" + self.wsfx, 2, nout, fm[-1], kin // fm[-1], "W1p", "W1dg"))
+        elif self.pool_type == "mlp":        # Conv1d(C, C, 1) weight [C][C][1] = a Linear with t_len 1
+            ls.append(PackedLayer("mlp.0.weight" + self.wsfx, 2, fm[-1], fm[-1], 1, "Wm0", "Wm0dg"))
         ls += [PackedLayer("enc_blocks.%d.conv.weight%s" % (l, self.wsfx), 0, fm[l], fm[l - 1], 0, "Wf%d" % l, "Wdg%d" % l)
                for l in range(self.nl - 1, 0, -1)]
         return ls
 
     # -- spectral norm ----------------------------------------------------------------------------
     SN_SLOTS = 5                    # up to 4 accumulating passes per optimiser step (WSEGAN) + 1 gradient-free pass
+    # the head's spectrally normalised tensors (discriminator.py:118-121,125-137)
+    HEAD_SN = {"none": ("fc.0.weight_orig", "fc.2.weight_orig", "fc.3.weight_orig"),
+               "conv": ("pool_conv.weight_orig", "fc.weight_orig"), "gmax": ("fc.weight_orig",),
+               "gavg": ("fc.weight_orig",), "mlp": ("mlp.0.weight_orig", "mlp.1.weight_orig")}
 
     def _sn_names(self):
-        return (["enc_blocks.%d.conv.weight_orig" % l for l in range(self.nl)] +
-                ["fc.0.weight_orig", "fc.2.weight_orig", "fc.3.weight_orig"])
+        return ["enc_blocks.%d.conv.weight_orig" % l for l in range(self.nl)] + list(self.HEAD_SN[self.pool_type])
 
     def _sn_state(self, name):
         """Spectral-norm state of one weight: the power-iteration vectors (u: the module's buffer itself; v: packed
@@ -1430,7 +1444,8 @@ class DiscriminatorEngine(_NetEngine):
         self._alpha_fixed = True
 
     def grad_chunks(self):
-        a = self.layers[0].numel + self.layers[1].numel
+        """[fc.0 | mlp.0 +] enc4 (complete once the last tower layer's weight gradient is enqueued) | the rest."""
+        a = sum(l.numel for l in self.layers[:2 if self.pool_type in ("none", "mlp") else 1])
         return [(0, a), (a, self.grad.numel() - a)]
 
     def pack(self):
@@ -1438,16 +1453,17 @@ class DiscriminatorEngine(_NetEngine):
         w0 = self.pview("enc_blocks.0.conv.weight" + self.wsfx)
         if self.snorm:
             w0 = w0 * self.sn_inv_sigma("enc_blocks.0.conv.weight_orig")
-            # the head's small normalised tensors, consumed by sg_fc_tail_fwd / _bwd
-            self.packed["fc2n"] = (self.pview("fc.2.weight_orig") * self.sn_inv_sigma("fc.2.weight_orig")).contiguous()
-            self.packed["fc3n"] = (self.pview("fc.3.weight_orig") * self.sn_inv_sigma("fc.3.weight_orig")).contiguous()
+            # the head's small normalised tensors, consumed by sg_fc_tail_fwd / _bwd or sg_dhead_fwd / _bwd
+            for nm in self.HEAD_SN[self.pool_type]:
+                if nm not in self.by_name:          # fc.0 / mlp.0: packed layers, emitted with their 1/sigma below
+                    self.packed[nm + "/n"] = (self.pview(nm) * self.sn_inv_sigma(nm)).contiguous()
         wcol = wave_col_weights(w0, dev)
         self.packed["Wcol0"] = wcol.half().contiguous()
         self.packed["WcolT0"] = wcol.t().to(GT).contiguous()
         self._mark_packed("small")
         for pl in self.layers:
             self.emit(pl, scale=self.sn_inv_sigma(pl.name) if self.snorm else None)
-            if pl.kind == 2:       # the Linear's operands are used as 2-D [nout][kin] / [kin][nout]
+            if pl.f_key == "W1p":  # fc.0's operands are used as 2-D [nout][kin] / [kin][nout]
                 self.packed["W1p"] = self.packed["W1p"].view(pl.nc, pl.kc)
                 self.packed["W1dg"] = self.packed["W1dg"].view(pl.kc, pl.nc)
 
@@ -1481,7 +1497,10 @@ class DiscriminatorEngine(_NetEngine):
         x0 = x0.contiguous().float()
         x1 = x1.contiguous().float()
         Lq = [L // 4 ** (l + 1) for l in range(nl)]
-        assert Lq[-1] * fm[-1] == self._param("fc.0.weight" + self.wsfx).shape[1], "D expects L = 16384"
+        if self.pool_type == "none":
+            assert Lq[-1] * fm[-1] == self._param("fc.0.weight" + self.wsfx).shape[1], "D expects L = 16384"
+        elif self.pool_type == "conv":
+            assert Lq[-1] == self._param("fc.weight" + self.wsfx).shape[1], "D expects L = 4^n_layers * pool_slen"
         if shifts_dev is not None and not wave_on_tensor_cores():
             raise _lib.SeganB200Error("device-resident phase shifts need the tensor-core waveform route")
 
@@ -1552,26 +1571,134 @@ class DiscriminatorEngine(_NetEngine):
                       halo, _p(hp[l]), _p(hpb[l]), None, st)
             if alias:
                 hpb[l] = hp[l]
-        # ---- FC head
-        kin = Lq[-1] * fm[-1]
-        acc = buf.get("d.fc0", (B, 256), F32, dev, zero=True)
-        self.wait_packed("W1p")
-        run_f(hp[-1], None, 1, 0, SG_F16, self.packed["W1p"], SG_F16, kin, 256,
-              tap_ranges("full", 0, kin, 256), acc, SG_F32, 1, 0, 0, 1, B, d_lo=0, d_hi=0, w_tap0=4,
-              ksplit=16, backend=self.backend)
-        z1 = buf.get("d.z1", (B, 256), F32, dev)
-        z2 = buf.get("d.z2", (B, 128), F32, dev)
-        logit = torch.empty(B, 1, dtype=F32, device=dev)
-        w2 = self.packed["fc2n"] if self.snorm else self.pview("fc.2.weight")
-        s3 = self.packed["fc3n"] if self.snorm else self.pview("fc.3.weight")
-        _lib.call("sg_fc_tail_fwd", _p(acc), _p(self.pview("fc.0.bias")), _p(self.pview("fc.1.weight")),
-                  _p(w2), _p(self.pview("fc.2.bias")), _p(s3),
-                  _p(self.pview("fc.4.weight")), _p(self.pview("fc.4.bias")), B, _p(z1), _p(z2), _p(logit), st)
+        if self.pool_type == "mlp":
+            logit, head = self._mlp_head_fwd(hp[-1], B, Lq[-1], buf)
+        elif self.pool_type != "none":
+            logit = torch.empty(B, 1, dtype=F32, device=dev)
+            head = self._pool_head_fwd(hp[-1], B, Lq[-1], buf, logit)
+        else:
+            # ---- FC head
+            kin = Lq[-1] * fm[-1]
+            acc = buf.get("d.fc0", (B, 256), F32, dev, zero=True)
+            self.wait_packed("W1p")
+            run_f(hp[-1], None, 1, 0, SG_F16, self.packed["W1p"], SG_F16, kin, 256,
+                  tap_ranges("full", 0, kin, 256), acc, SG_F32, 1, 0, 0, 1, B, d_lo=0, d_hi=0, w_tap0=4,
+                  ksplit=16, backend=self.backend)
+            z1 = buf.get("d.z1", (B, 256), F32, dev)
+            z2 = buf.get("d.z2", (B, 128), F32, dev)
+            logit = torch.empty(B, 1, dtype=F32, device=dev)
+            w2 = self.packed["fc.2.weight_orig/n"] if self.snorm else self.pview("fc.2.weight")
+            s3 = self.packed["fc.3.weight_orig/n"] if self.snorm else self.pview("fc.3.weight")
+            _lib.call("sg_fc_tail_fwd", _p(acc), _p(self.pview("fc.0.bias")), _p(self.pview("fc.1.weight")),
+                      _p(w2), _p(self.pview("fc.2.bias")), _p(s3),
+                      _p(self.pview("fc.4.weight")), _p(self.pview("fc.4.bias")), B, _p(z1), _p(z2), _p(logit), st)
+            head = dict(z1=z1, z2=z2, acc=acc, w2=w2, s3=s3)
         self.packs_consumed()
-        ctx = dict(x0=x0, x1=x1, B=B, L=L, Lq=Lq, a=a, hp=hp, hpb=hpb, colb=colb0, ss=ss, mi=mi, z1=z1, z2=z2,
-                   logit=logit, lane=lane, shifts_dev=shifts_dev, acc=acc, w2=w2, s3=s3, sn_slot=sn_slot,
-                   shifts=[int(s) for s in shifts])
+        ctx = dict(x0=x0, x1=x1, B=B, L=L, Lq=Lq, a=a, hp=hp, hpb=hpb, colb=colb0, ss=ss, mi=mi,
+                   logit=logit, lane=lane, shifts_dev=shifts_dev, sn_slot=sn_slot,
+                   shifts=[int(s) for s in shifts], **head)
         return logit, ctx
+
+    # -- pooled heads (pool_type 'conv' / 'gmax' / 'gavg') --------------------------------------------
+    def _head_weights(self):
+        """(pool_conv weight, pool_conv bias, fc weight, fc bias) as the head kernels read them: the spectrally
+        normalised copies made by pack() where norm_type='snorm'; the pool_conv entries are None without one."""
+        w = lambda nm: self.packed[nm + "_orig/n"] if self.snorm else self.pview(nm)
+        pw = w("pool_conv.weight") if self.pool_type == "conv" else None
+        pb = self.pview("pool_conv.bias") if self.pool_type == "conv" else None
+        return pw, pb, w("fc.weight"), self.pview("fc.bias")
+
+    def _pool_head_fwd(self, h, B, lq, buf, logit):
+        """h: the last tower activation [B][lq][C] fp16.  Fills logit (B, 1); returns the head's saved tensors."""
+        dev, c = h.device, self.fmaps[-1]
+        kind = DHEAD_KINDS[self.pool_type]
+        pw, pb, fw, fb = self._head_weights()
+        pooled = buf.get("d.pooled", (B, lq if kind == SG_DHEAD_CONV else c), F32, dev)
+        argmax = buf.get("d.argmax", (B, c), torch.int32, dev) if kind == SG_DHEAD_GMAX else None
+        _lib.call("sg_dhead_fwd", kind, _p(h), B, lq, c, _p(pw), _p(pb), _p(fw), _p(fb), _p(pooled), _p(argmax),
+                  _p(logit), _stream())
+        return dict(pooled=pooled, argmax=argmax, pw=pw, fw=fw)
+
+    def _mlp_head_fwd(self, h, B, lq, buf):
+        """pool_type 'mlp' on the last tower activation h [B][lq][C] fp16: logits (B, 1, lq) and the saved tensors."""
+        dev, c, rows, st = h.device, self.fmaps[-1], B * lq, _stream()
+        pl = self.by_name["mlp.0.weight" + self.wsfx]
+        z = buf.get("d.mlp.z", (B, lq, c), F16, dev)
+        self.wait_packed(pl.f_key)
+        run_f(h, None, rows, 0, SG_F16, self.packed[pl.f_key], SG_F16, c, c, tap_ranges("full", 0, c, c), z, SG_F16,
+              rows, 0, 0, rows, 1, bias=self.pview("mlp.0.bias"), bias_mod=c, d_lo=0, d_hi=0, w_tap0=4,
+              backend=self.backend)
+        slope = self.packed["mlp.1.weight_orig/n"] if self.snorm else self.pview("mlp.1.weight")
+        hm = buf.get("d.mlp.h", (B, lq, c), F16, dev)
+        _lib.call("sg_act_fwd", _p(z), SG_F16, B, lq, c, None, _p(slope), ACT_PRELU, 0, None, 0, _p(hm), None, None, st)
+        logit = torch.empty(B, 1, lq, dtype=F32, device=dev)
+        _lib.call("sg_dhead_fwd", SG_DHEAD_MLP, _p(hm), B, lq, c, _p(self.pview("mlp.2.weight")),
+                  _p(self.pview("mlp.2.bias")), None, None, None, None, _p(logit), st)
+        return logit, dict(mlp_z=z, mlp_h=hm, mlp_slope=slope)
+
+    def _mlp_head_bwd(self, ctx, target, weight, param_grads, loss_out, g_logit, g_h, buf, slot, side):
+        """Loss + backward of the mlp head: mlp.2 and the loss in sg_dhead_bwd, the PReLU through the tower's
+        activation backward (its slope and mlp.0's bias from the reduction), mlp.0's weight gradient on the side
+        stream and its data gradient into g_h."""
+        B, lq, c, st = ctx["B"], ctx["Lq"][-1], self.fmaps[-1], _stream()
+        dev, rows, sn = g_h.device, B * lq, self.snorm
+        pl = self.by_name["mlp.0.weight" + self.wsfx]
+        g_hm = buf.get("d.mlp.gh", (B, lq, c), GT, dev)
+        gv = (lambda n: _p(self.gview(n))) if param_grads else (lambda n: None)
+        _lib.call("sg_dhead_bwd", SG_DHEAD_MLP, _p(ctx["mlp_h"]), B, lq, c, _p(self.pview("mlp.2.weight")), None, None,
+                  None, _p(ctx["logit"]), _p(g_logit), float(target), float(weight), _p(loss_out), _p(g_hm),
+                  gv("mlp.2.weight"), gv("mlp.2.bias"), None, None, float(LOSS_SCALE), st)
+        red = buf.get("d.mlp.red", (SL, 3, c), F64, dev, zero=True)
+        g_z = buf.get("d.mlp.gz", (B, lq, c), GT, dev)
+        _lib.call("sg_act_bwd_reduce", _p(g_hm), c, 0, 0, None, None, 0, _p(ctx["mlp_z"]), SG_F16, B, lq, c, None, None,
+                  _p(ctx["mlp_slope"]), ACT_PRELU, _p(red), _p(g_z), st)
+        taps = tap_ranges("full", 0, c, c)
+        if param_grads:
+            g_slope = buf.get("d.sng.mlp.1", (c,), F32, dev, zero=True) if sn else self.gview("mlp.1.weight")
+            # red is [SL][3][C] (sg_stat_grads strides its slices by n_stats): 3 statistics, the third unused
+            _lib.call("sg_stat_grads", _p(red), c, 3, _p(g_slope), _p(self.gview("mlp.0.bias")), None, st)
+            osc = None
+            if sn:
+                self._sn_fix_small("mlp.1.weight_orig", g_slope, slot)
+                stt = self._sn_state(pl.name)
+                _lib.call("sg_snorm_coef", _p(red), _p(self.pview("mlp.0.bias")), c, _p(stt["scal"][slot]),
+                          _p(stt["coef"][slot:slot + 1]), st)
+                osc = stt["scal"][slot][3:4]
+            with on_side(side):
+                run_w(g_z, rows, GS, ctx["hpb"][-1], None, rows, 0, GS, c, c, taps, self.mgrad(pl), 1, d_lo=0, d_hi=0,
+                      dw_tap0=4, ksplit=wgrad_ksplit(rows, 0, taps, c, c, 0, 0), backend=self.backend, out_scale=osc)
+        run_f(g_z, None, rows, 0, GS, self.packed[pl.dg_key], GS, c, c, taps, g_h, GS, rows, 0, 0, rows, 1, d_lo=0,
+              d_hi=0, w_tap0=4, backend=self.backend)
+
+    def _pool_head_bwd(self, ctx, target, weight, param_grads, loss_out, g_logit, g_h, buf, slot):
+        """Loss + backward of a pooled head into g_h (every element written) and, with param_grads, the head's
+        parameter gradients into the bucket (snorm: through per-pass scratch gradients and sg_snorm_grad)."""
+        B, lq, c = ctx["B"], ctx["Lq"][-1], self.fmaps[-1]
+        kind = DHEAD_KINDS[self.pool_type]
+        conv = kind == SG_DHEAD_CONV
+        g = {}
+        if param_grads:
+            for nm in ("pool_conv.weight", "pool_conv.bias", "fc.weight", "fc.bias"):
+                if not conv and nm.startswith("pool_conv"):
+                    continue
+                if self.snorm and nm.endswith("weight"):
+                    g[nm] = buf.get("d.sng." + nm, self.index[nm + "_orig"][2], F32, ctx["x0"].device, zero=True)
+                else:
+                    g[nm] = self.gview(nm)
+        _lib.call("sg_dhead_bwd", kind, _p(ctx["hp"][-1]), B, lq, c, _p(ctx["pw"]), _p(ctx["fw"]), _p(ctx["pooled"]),
+                  _p(ctx["argmax"]), _p(ctx["logit"]), _p(g_logit), float(target), float(weight), _p(loss_out),
+                  _p(g_h), _p(g.get("pool_conv.weight")), _p(g.get("pool_conv.bias")), _p(g.get("fc.weight")),
+                  _p(g.get("fc.bias")), float(LOSS_SCALE), _stream())
+        if param_grads and self.snorm:
+            for nm in self.HEAD_SN[self.pool_type]:
+                self._sn_fix_small(nm, g[nm[:-len("_orig")]], slot)
+
+    def _sn_fix_small(self, nm, scratch, slot):
+        """scratch gradient w.r.t. the normalised small tensor `nm` -> gradient w.r.t. weight_orig, into the bucket."""
+        stt = self._sn_state(nm)
+        _lib.call("sg_snorm_grad", _p(scratch), _p(self.pview(nm)), 1, stt["nc"], stt["kc"], _p(stt["u_p"][slot]),
+                  _p(stt["v_p"][slot]), _p(stt["scal"][slot]), _p(stt["work"][stt["nc"]:]), _stream())
+        self.gview(nm).add_(scratch)
 
     def backward(self, ctx, target, weight=1.0, param_grads=True, input_grad=None, loss_out=None, g_logit=None,
                  input_grad1=None, reducer=None, reduce_now=True):
@@ -1592,52 +1719,55 @@ class DiscriminatorEngine(_NetEngine):
         B, L, Lq = ctx["B"], ctx["L"], ctx["Lq"]
         a, hp, ss, mi, shifts = ctx["a"], ctx["hp"], ctx["ss"], ctx["mi"], ctx["shifts"]
         dev = ctx["x0"].device
-        kin = Lq[-1] * fm[-1]
-        g_z1 = buf.get("d.gz1", (B, 256), GT, dev)
-        ws = buf.get("d.fcws", (B * (1 + 128 + 256 + 256),), F32, dev)
+        fc_head = self.pool_type == "none"
+        if fc_head:
+            kin = Lq[-1] * fm[-1]
+            g_z1 = buf.get("d.gz1", (B, 256), GT, dev)
+            ws = buf.get("d.fcws", (B * (1 + 128 + 256 + 256),), F32, dev)
         gv = (lambda n: _p(gview(n))) if param_grads else (lambda n: None)
         sn, slot, wsfx = self.snorm, ctx.get("sn_slot"), self.wsfx
         sn_small = {}             # snorm: per-pass scratch gradients of the small normalised tensors
         if sn and param_grads:
-            for nm in ("fc.2.weight_orig", "fc.3.weight_orig", "enc_blocks.0.conv.weight_orig"):
+            head_sn = ("fc.2.weight_orig", "fc.3.weight_orig") if fc_head else ()
+            for nm in head_sn + ("enc_blocks.0.conv.weight_orig",):
                 sn_small[nm] = buf.get("d.sng." + nm, self.index[nm][2], F32, dev, zero=True)
-        g_w2 = _p(sn_small["fc.2.weight_orig"]) if sn_small else gv("fc.2.weight")
-        g_s3 = _p(sn_small["fc.3.weight_orig"]) if sn_small else gv("fc.3.weight")
-        _lib.call("sg_fc_tail_bwd", _p(ctx["z1"]), _p(ctx["z2"]), _p(ctx["logit"]), _p(g_logit), float(target),
-                  float(weight),
-                  _p(self.pview("fc.1.weight")), _p(ctx["w2"]), _p(ctx["s3"]),
-                  _p(self.pview("fc.4.weight")), B, _p(loss_out), _p(g_z1), _p(ws),
-                  gv("fc.0.bias"), gv("fc.1.weight"), g_w2, gv("fc.2.bias"), g_s3,
-                  gv("fc.4.weight"), gv("fc.4.bias"), float(LOSS_SCALE), st)
-
-        def sn_fix_small(nm):
-            """scratch gradient w.r.t. the normalised small tensor -> gradient w.r.t. weight_orig, into the bucket."""
-            stt = self._sn_state(nm)
-            _lib.call("sg_snorm_grad", _p(sn_small[nm]), _p(self.pview(nm)), 1, stt["nc"], stt["kc"], _p(stt["u_p"][slot]),
-                      _p(stt["v_p"][slot]), _p(stt["scal"][slot]), _p(stt["work"][stt["nc"]:]), _stream())
-            gview(nm).add_(sn_small[nm])
-        if sn_small:
-            sn_fix_small("fc.2.weight_orig")
-            sn_fix_small("fc.3.weight_orig")
         # weight-gradient chain (wgrad GEMM + unpack) of every layer: side stream 0, next to the
         # data-gradient chain (dgrad GEMM -> BatchNorm/PReLU backward) on the caller's stream
         side = side_stream(dev, 3 if lane == 1 else 0) if param_grads else None
-        if param_grads:
-            fc0 = self.by_name["fc.0.weight" + wsfx]
-            dw1 = self.mgrad(fc0)
-            osc = None
-            if sn:
-                # <dL/dW~, W~> of fc.0 = <g_z1, fc0 output without bias>; coefficient of this pass's sigma term
-                stt = self._sn_state(fc0.name)
-                gz1f = ws[B * 129:B * 129 + B * 256]
-                stt["coef"][slot] = (gz1f * ctx["acc"].reshape(-1)).sum() * stt["scal"][slot][3]
-                osc = stt["scal"][slot][3:4]
-            with on_side(side):
-                run_w(g_z1, 1, GS, ctx["hpb"][-1], None, 1, 0, GS, kin, 256, tap_ranges("full", 0, kin, 256),
-                      dw1, B, d_lo=0, d_hi=0, dw_tap0=4, ksplit=1, backend=self.backend, out_scale=osc)
-        g_h = buf.get("d.gh%d" % (nl - 1), (B, Lq[-1], fm[-1]), GT, dev)
-        run_f(g_z1, None, 1, 0, GS, self.packed["W1dg"], GS, 256, kin, tap_ranges("full", 0, 256, kin),
-              g_h, GS, 1, 0, 0, 1, B, d_lo=0, d_hi=0, w_tap0=4, backend=self.backend)
+        if not fc_head:
+            g_h = buf.get("d.gh%d" % (nl - 1), (B, Lq[-1], fm[-1]), GT, dev)
+            if self.pool_type == "mlp":
+                self._mlp_head_bwd(ctx, target, weight, param_grads, loss_out, g_logit, g_h, buf, slot, side)
+            else:
+                self._pool_head_bwd(ctx, target, weight, param_grads, loss_out, g_logit, g_h, buf, slot)
+        else:
+            g_w2 = _p(sn_small["fc.2.weight_orig"]) if sn_small else gv("fc.2.weight")
+            g_s3 = _p(sn_small["fc.3.weight_orig"]) if sn_small else gv("fc.3.weight")
+            _lib.call("sg_fc_tail_bwd", _p(ctx["z1"]), _p(ctx["z2"]), _p(ctx["logit"]), _p(g_logit), float(target),
+                      float(weight),
+                      _p(self.pview("fc.1.weight")), _p(ctx["w2"]), _p(ctx["s3"]),
+                      _p(self.pview("fc.4.weight")), B, _p(loss_out), _p(g_z1), _p(ws),
+                      gv("fc.0.bias"), gv("fc.1.weight"), g_w2, gv("fc.2.bias"), g_s3,
+                      gv("fc.4.weight"), gv("fc.4.bias"), float(LOSS_SCALE), st)
+            if sn_small:
+                self._sn_fix_small("fc.2.weight_orig", sn_small["fc.2.weight_orig"], slot)
+                self._sn_fix_small("fc.3.weight_orig", sn_small["fc.3.weight_orig"], slot)
+            if param_grads:
+                fc0 = self.by_name["fc.0.weight" + wsfx]
+                dw1 = self.mgrad(fc0)
+                osc = None
+                if sn:
+                    # <dL/dW~, W~> of fc.0 = <g_z1, fc0 output without bias>; coefficient of this pass's sigma term
+                    stt = self._sn_state(fc0.name)
+                    gz1f = ws[B * 129:B * 129 + B * 256]
+                    stt["coef"][slot] = (gz1f * ctx["acc"].reshape(-1)).sum() * stt["scal"][slot][3]
+                    osc = stt["scal"][slot][3:4]
+                with on_side(side):
+                    run_w(g_z1, 1, GS, ctx["hpb"][-1], None, 1, 0, GS, kin, 256, tap_ranges("full", 0, kin, 256),
+                          dw1, B, d_lo=0, d_hi=0, dw_tap0=4, ksplit=1, backend=self.backend, out_scale=osc)
+            g_h = buf.get("d.gh%d" % (nl - 1), (B, Lq[-1], fm[-1]), GT, dev)
+            run_f(g_z1, None, 1, 0, GS, self.packed["W1dg"], GS, 256, kin, tap_ranges("full", 0, 256, kin),
+                  g_h, GS, 1, 0, 0, 1, B, d_lo=0, d_hi=0, w_tap0=4, backend=self.backend)
         tmp = buf.get("d.cstmp", (SL * 2048,), F64, dev)
         reds = stat_arena(buf, "d.red", [(SL, 3, fm[l]) for l in range(nl)], dev)
         for l in range(nl - 1, -1, -1):
@@ -1689,13 +1819,15 @@ class DiscriminatorEngine(_NetEngine):
                               backend=self.backend)
                         _lib.call("sg_wave_wgrad_fold", _p(dwq), 2, _p(g_w0), _stream())
                         if sn_small:
-                            sn_fix_small("enc_blocks.0.conv.weight_orig")
+                            self._sn_fix_small("enc_blocks.0.conv.weight_orig",
+                                               sn_small["enc_blocks.0.conv.weight_orig"], slot)
                 elif param_grads:
                     with on_side(side):
                         _lib.call("sg_wave_conv_wgrad", _p(ctx["x0"]), _p(ctx["x1"]), 2, B, L, shifts[0], _p(g_a),
                                   cout, _p(g_w0), None, _stream())
                         if sn_small:
-                            sn_fix_small("enc_blocks.0.conv.weight_orig")
+                            self._sn_fix_small("enc_blocks.0.conv.weight_orig",
+                                               sn_small["enc_blocks.0.conv.weight_orig"], slot)
                 if (input_grad is not None or input_grad1 is not None) and wave_on_tensor_cores():
                     P2 = buf.get("d.P2", (B, Lq[0], 64), GT, dev)
                     run_f(g_a, None, Lq[0], 0, GS, self.packed["WcolT0"], GS, 64, 64,

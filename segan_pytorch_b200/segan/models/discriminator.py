@@ -2,7 +2,8 @@
 
 conv -> BatchNorm1d -> PReLU tower with the random circular phase shift before every layer
 (two python-`random` draws per layer, also in eval mode -- discriminator.py:160-172) and the
-16384-256-128-1 PReLU head.  Arithmetic: segan_pytorch_b200.engine.DiscriminatorEngine."""
+16384-256-128-1 PReLU head (pool_type 'none'), or one of the pooled heads 'conv' / 'gmax' / 'gavg' / 'mlp'
+(discriminator.py:122-146; 'mlp' gives one logit per position, (B, 1, L / 4^n_layers)).  Arithmetic: segan_pytorch_b200.engine.DiscriminatorEngine."""
 import random
 
 import torch
@@ -80,6 +81,7 @@ class Discriminator(Model):
             self.enc_blocks.append(GConv1DBlock(ninp, fmap, kwidth, stride=pool, bias=bias, norm_type=norm_type))
             ninp = fmap
         self.pool_type = pool_type
+        self.pool_slen = pool_slen                     # positions after the tower (16 for L = 16384)
         if pool_type == 'none':
             pool_slen *= fmaps[-1]
             self.fc = nn.Sequential(
@@ -93,9 +95,31 @@ class Discriminator(Model):
                 torch.nn.utils.spectral_norm(self.fc[0])
                 torch.nn.utils.spectral_norm(self.fc[2])
                 torch.nn.utils.spectral_norm(self.fc[3])
+        elif pool_type == 'conv':                      # discriminator.py:122-127: pool_slen is NOT scaled by C here
+            self.pool_conv = nn.Conv1d(fmaps[-1], 1, 1)
+            self.fc = nn.Linear(pool_slen, 1)
+            if norm_type == 'snorm':
+                torch.nn.utils.spectral_norm(self.pool_conv)
+                torch.nn.utils.spectral_norm(self.fc)
+        elif pool_type in ('gmax', 'gavg'):            # discriminator.py:128-137 (Linear's third argument: bias)
+            if pool_type == 'gmax':
+                self.gmax = nn.AdaptiveMaxPool1d(1)
+            else:
+                self.gavg = nn.AdaptiveAvgPool1d(1)
+            self.fc = nn.Linear(fmaps[-1], 1, 1)
+            if norm_type == 'snorm':
+                torch.nn.utils.spectral_norm(self.fc)
+        elif pool_type == 'mlp':                       # discriminator.py:138-146: mlp.2 is not normalised
+            self.mlp = nn.Sequential(
+                nn.Conv1d(fmaps[-1], fmaps[-1], 1),
+                nn.PReLU(fmaps[-1]),
+                nn.Conv1d(fmaps[-1], 1, 1)
+            )
+            if norm_type == 'snorm':
+                torch.nn.utils.spectral_norm(self.mlp[0])
+                torch.nn.utils.spectral_norm(self.mlp[1])
         else:
-            raise NotImplementedError("pool_type %r is a SURVEY.md 8(f)-N4 'next' row; only 'none' is built"
-                                      % (pool_type,))
+            raise TypeError('Unrecognized pool type: ', pool_type)
         self.fmaps = list(fmaps)
         self.bias = bias
         self.norm_type = norm_type
@@ -107,7 +131,7 @@ class Discriminator(Model):
     def engine(self):
         if not self._served:
             raise NotImplementedError("this Discriminator configuration is outside the built hot path "
-                                      "(SEGAN+ defaults: 2 input channels, bnorm, k=31, stride 4, pool 'none')")
+                                      "(SEGAN+ defaults: 2 input channels, bnorm or snorm, k=31, stride 4)")
         if self._engine is None:
             self._engine = _engine.DiscriminatorEngine(self)
         return self._engine
@@ -141,6 +165,8 @@ class Discriminator(Model):
             y, ectx = eng.forward(x[:, 0:1, :].contiguous(), x[:, 1:2, :].contiguous(), shifts,
                                   training=self.training)
         int_act = _LazyActs(eng, ectx)
+        if self.pool_type == 'conv':        # pool_conv output (B, Lq), discriminator.py:176-178; its buffer is reused
+            int_act['avg_conv_h'] = ectx["pooled"].clone()
         int_act['logit'] = y
         return y, int_act
 

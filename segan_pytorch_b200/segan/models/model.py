@@ -570,6 +570,16 @@ class SEGAN(Model):
             r = self.__dict__['_grad_reducers'] = (GradReducer(de), GradReducer(ge))
         return r
 
+    def _check_d_logits(self, B):
+        """SEGAN's losses compare D's logits, flattened, with B labels (model.py:298,305,316).  pool_type='mlp' gives
+        B * Lq logits, which the reference rejects in its first step; refuse it before training anything."""
+        if getattr(self.D, 'pool_type', 'none') == 'mlp':
+            lq = self.D.pool_slen
+            raise RuntimeError("SEGAN cannot train a Discriminator with pool_type='mlp': it gives one logit per "
+                               "position, B * Lq = %d logits against B = %d labels (the reference fails at "
+                               "model.py:298 with 'The size of tensor a (%d) must match the size of tensor b (%d)'); "
+                               "WSEGAN (--wsegan) trains it" % (B * lq, B, B * lq, B))
+
     def train_step(self, clean, noisy, Gopt, Dopt, l1_weight, z=None, shifts3=None, losses=None):
         """clean / noisy: (B,1,L) fp32 cuda.  Returns the device tensor of the four losses
         [d_real, d_fake, g_adv, g_l1] (no host sync).
@@ -579,6 +589,7 @@ class SEGAN(Model):
         data-parallel run sit between them) and replayed: the ~300 launches of a step then cost no host
         time and the side-stream schedule (engine.OVERLAP) becomes real concurrency on the device.  The
         per-step phase shifts live in a small device table the host rewrites before each replay."""
+        self._check_d_logits(clean.shape[0])
         ge, de = self.G.engine, self.D.engine
         B, _, L = clean.shape
         dev = clean.device
@@ -824,6 +835,7 @@ class SEGAN(Model):
               device='cuda'):
         """Train the SEGAN (model.py:230-437): same loop structure, logging line and checkpoint
         cadence.  `criterion` must be nn.MSELoss (LSGAN); it is fused into the D head backward."""
+        self._check_d_logits(opts.batch_size)
         if not isinstance(criterion, nn.MSELoss):
             raise NotImplementedError("SEGAN.train is built for the LSGAN criterion nn.MSELoss (train.py:94)")
         rank0 = _dist() is None or _dist().get_rank() == 0
