@@ -329,6 +329,11 @@ int sg_fc_tail_bwd(const float* z1, const float* z2, const float* logit,
 /* G regression loss (model.py:318): loss = w * mean|y - clean| ; gy (+)= grad_scale*w*sign(y-clean)/(B*L) */
 int sg_l1_loss_bwd(const float* y, const float* clean, int64_t n, float weight, float* loss_out,
                    float* gy, int accumulate, float grad_scale /* multiplies gy only */, void* stream);
+/* --reg_loss mse_loss (model.py:79,318): loss = w * mean (y - clean)^2 ; gy (+)= grad_scale*2w*(y-clean)/(B*L).
+ * Both losses add to *loss_out (may be NULL), summed in a fixed order (the same bits run to run); launches of the
+ * two must not overlap each other on one device (per-device partial sums). */
+int sg_mse_loss_bwd(const float* y, const float* clean, int64_t n, float weight, float* loss_out,
+                    float* gy, int accumulate, float grad_scale /* multiplies gy only */, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * WSEGAN's spectral term (model.py:638-653): pow_weight * mean| 10 log10(|STFT(G)|^2 + 1e-19) - 10 log10(|STFT(clean)|^2
@@ -402,6 +407,9 @@ int sg_snorm_rank1(float* dwp, int n_taps, int nc, int kc, int n_pass, const flo
 int sg_wave_wgrad_fold(float* dwq /* the blocks read are cleared */, int cin, float* dw, void* stream);
 int sg_last_deconv_wgrad_fold(float* dwq /* the blocks read are cleared */, int half, const float* w, const float* alpha, float* dw,
                               float* dalpha, void* stream);
+/* the same fold for a Generator without skips (skip=False): dwq[2][64][2][cin] (s, k-slot, s', c) -> dW[cin][1][31]
+ * += dwq[0][k][0][c] + dwq[1][k][1][c]; no alpha */
+int sg_last_deconv_wgrad_fold_1src(float* dwq /* the blocks read are cleared */, int cin, float* dw, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Convolutional skip connection (GSkip skip_type='conv', generator.py:43-49): nn.Conv1d(C, C, K, stride 1,

@@ -76,6 +76,7 @@ _SIGS = {
     "sg_fc_tail_fwd": [_vp] * 8 + [_i, _vp, _vp, _vp, _vp],
     "sg_fc_tail_bwd": [_vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp] + [_vp] * 7 + [_f, _vp],
     "sg_l1_loss_bwd": [_vp, _vp, _i64, _f, _vp, _vp, _i, _f, _vp],
+    "sg_mse_loss_bwd": [_vp, _vp, _i64, _f, _vp, _vp, _i, _f, _vp],
     "sg_rmsprop_step": [_vp, _vp, _vp, _i64, _f, _f, _f, _f, _i, _vp],
     "sg_adam_step": [_vp, _vp, _vp, _vp, _i64, _f, _f, _f, _f, _i, _f, _i, _vp],
     "sg_emit_operands": [_vp, _i, _i, _i, _vp, _i, _vp, _vp, _i, _i, _vp, _vp],
@@ -86,6 +87,7 @@ _SIGS = {
     "sg_alpha_grad": [_vp, _vp, _i, _i, _i, _vp, _i, _vp, _vp],
     "sg_wave_wgrad_fold": [_vp, _i, _vp, _vp],
     "sg_last_deconv_wgrad_fold": [_vp, _i, _vp, _vp, _vp, _vp, _vp],
+    "sg_last_deconv_wgrad_fold_1src": [_vp, _i, _vp, _vp],
     "sg_deemphasis": [_vp, _i64, _f, _vp, _vp],
     "sg_preemphasis": [_vp, _i64, _f, _vp, _vp],
     "sg_pcm16_to_wave": [_vp, _vp, _i64, _i, _f, _vp, _vp, _vp],

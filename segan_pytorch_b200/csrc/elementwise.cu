@@ -797,20 +797,57 @@ fc_tail_bwd_params_kernel(const float* __restrict__ z1, const float* __restrict_
   }
 }
 
-__global__ void l1_loss_bwd_kernel(const float* __restrict__ y, const float* __restrict__ clean, int64_t n,
-                                   float weight, float* __restrict__ loss_out, float* __restrict__ gy,
-                                   int accumulate, float grad_scale) {
+// G regression loss and its gradient, per element d = y - clean:  REG_L1: |d|, w/n sign(d)  |  REG_MSE: d^2, 2 w/n d.
+// The loss is summed deterministically: every block stores its partial (fixed thread order), the last block to
+// finish adds the partials up in block order.  The partials and the arrival counter are per device, so launches
+// of this kernel must not overlap one another (they run on one stream; the counter is reset for the next launch).
+enum { REG_L1 = 0, REG_MSE = 1 };
+constexpr int REG_BLOCKS = 2 * NUM_SMS;
+__device__ float g_reg_partial[REG_BLOCKS];
+__device__ unsigned int g_reg_arrived;
+
+template <int TERM>
+__global__ void __launch_bounds__(256) reg_loss_bwd_kernel(const float* __restrict__ y,
+                                                           const float* __restrict__ clean, int64_t n, float weight,
+                                                           float* __restrict__ loss_out, float* __restrict__ gy,
+                                                           int accumulate, float grad_scale) {
+  __shared__ float warp_part[8];
+  __shared__ bool last;
   float s = 0.f;
   const float lscale = weight / (float)n;
   const float gscale = lscale * grad_scale;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const float d = y[i] - clean[i];
-    s += fabsf(d);
-    const float g = d > 0.f ? gscale : (d < 0.f ? -gscale : 0.f);
+    float g;
+    if (TERM == REG_L1) {
+      s += fabsf(d);
+      g = d > 0.f ? gscale : (d < 0.f ? -gscale : 0.f);
+    } else {
+      s = fmaf(d, d, s);
+      g = 2.f * gscale * d;
+    }
     if (gy) gy[i] = accumulate ? gy[i] + g : g;
   }
   s = warp_sum(s);
-  if ((threadIdx.x & 31) == 0 && loss_out) atomicAdd(loss_out, s * lscale);
+  if ((threadIdx.x & 31) == 0) warp_part[threadIdx.x >> 5] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float b = 0.f;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) b += warp_part[w];
+    g_reg_partial[blockIdx.x] = b;
+    __threadfence();
+    last = atomicAdd(&g_reg_arrived, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (last && threadIdx.x < 32) {
+    float t = 0.f;
+    for (int b = threadIdx.x; b < (int)gridDim.x; b += 32) t += __ldcg(g_reg_partial + b);
+    t = warp_sum(t);
+    if (threadIdx.x == 0) {
+      if (loss_out) *loss_out += t * lscale;
+      g_reg_arrived = 0;
+    }
+  }
 }
 
 // ---- streaming-kernel variants (runtime tuning knobs, one per kernel family) -----------------
@@ -1123,7 +1160,14 @@ extern "C" int sg_fc_tail_bwd(const float* z1, const float* z2, const float* log
 
 extern "C" int sg_l1_loss_bwd(const float* y, const float* clean, int64_t n, float weight, float* loss_out,
                               float* gy, int accumulate, float grad_scale, void* stream) {
-  l1_loss_bwd_kernel<<<2 * NUM_SMS, 256, 0, ST>>>(y, clean, n, weight, loss_out, gy, accumulate, grad_scale);
+  reg_loss_bwd_kernel<REG_L1><<<REG_BLOCKS, 256, 0, ST>>>(y, clean, n, weight, loss_out, gy, accumulate, grad_scale);
+  SG_CHECK_LAUNCH();
+  return SG_OK;
+}
+
+extern "C" int sg_mse_loss_bwd(const float* y, const float* clean, int64_t n, float weight, float* loss_out,
+                               float* gy, int accumulate, float grad_scale, void* stream) {
+  reg_loss_bwd_kernel<REG_MSE><<<REG_BLOCKS, 256, 0, ST>>>(y, clean, n, weight, loss_out, gy, accumulate, grad_scale);
   SG_CHECK_LAUNCH();
   return SG_OK;
 }

@@ -316,31 +316,33 @@ __global__ void wave_wgrad_fold_kernel(float* __restrict__ dwq, int cin, float* 
   *p1 = 0.f;
   atomicAdd(dw + i, v);
 }
-//   last deconv (Cout = 1, alpha folded into its effective weight): dwq[2][64][2][2][half] (s, k-slot, source,
+//   last deconv (Cout = 1, alpha folded into its effective weight): dwq[2][64][NSRC][2][half] (s, k-slot, source,
 //   s', c); dWeff[src*half + c][k] = dwq[0][k][src][0][c] + dwq[1][k][src][1][c]; dW += dWeff (* alpha for the skip
-//   half), dalpha[c] += sum_k dWeff[half + c][k] * W[half + c][k]
+//   half), dalpha[c] += sum_k dWeff[half + c][k] * W[half + c][k].  NSRC = 2: cat(decoder, skip); NSRC = 1: the
+//   decoder output alone (no skips: no alpha, w / alpha / dalpha unused)
+template <int NSRC>
 __global__ void last_deconv_wgrad_fold_kernel(float* __restrict__ dwq, int half, const float* __restrict__ w,
                                               const float* __restrict__ alpha, float* __restrict__ dw,
                                               float* __restrict__ dalpha) {
-  const int ch = blockIdx.x * blockDim.x + threadIdx.x;       // channel of cat(decoder, skip): [0, 2*half)
-  if (ch >= 2 * half) return;
+  const int ch = blockIdx.x * blockDim.x + threadIdx.x;       // channel of cat(decoder, skip): [0, NSRC*half)
+  if (ch >= NSRC * half) return;
   const int src = ch / half, c = ch % half;
   float da = 0.f;
   for (int k = 0; k < KW; ++k) {
-    float* p0 = dwq + ((((int64_t)0 * 64 + k) * 2 + src) * 2 + 0) * half + c;
-    float* p1 = dwq + ((((int64_t)1 * 64 + k) * 2 + src) * 2 + 1) * half + c;
+    float* p0 = dwq + ((((int64_t)0 * 64 + k) * NSRC + src) * 2 + 0) * half + c;
+    float* p1 = dwq + ((((int64_t)1 * 64 + k) * NSRC + src) * 2 + 1) * half + c;
     const float v = *p0 + *p1;
     *p0 = 0.f;
     *p1 = 0.f;
     const int64_t wi = (int64_t)ch * KW + k;
-    if (src == 1) {
+    if (NSRC == 2 && src == 1) {
       da = fmaf(v, w[wi], da);
       atomicAdd(dw + wi, v * alpha[c]);
     } else {
       atomicAdd(dw + wi, v);
     }
   }
-  if (src == 1 && dalpha) atomicAdd(dalpha + c, da);
+  if (NSRC == 2 && src == 1 && dalpha) atomicAdd(dalpha + c, da);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -532,7 +534,14 @@ extern "C" int sg_wave_wgrad_fold(float* dwq, int cin, float* dw, void* stream) 
 extern "C" int sg_last_deconv_wgrad_fold(float* dwq, int half, const float* w, const float* alpha, float* dw,
                                          float* dalpha, void* stream) {
   SG_CHECK_ARG(dwq && w && alpha && dw && half > 0);
-  last_deconv_wgrad_fold_kernel<<<(2 * half + 127) / 128, 128, 0, ST>>>(dwq, half, w, alpha, dw, dalpha);
+  last_deconv_wgrad_fold_kernel<2><<<(2 * half + 127) / 128, 128, 0, ST>>>(dwq, half, w, alpha, dw, dalpha);
+  SG_CHECK_LAUNCH();
+  return SG_OK;
+}
+
+extern "C" int sg_last_deconv_wgrad_fold_1src(float* dwq, int cin, float* dw, void* stream) {
+  SG_CHECK_ARG(dwq && dw && cin > 0);
+  last_deconv_wgrad_fold_kernel<1><<<(cin + 127) / 128, 128, 0, ST>>>(dwq, cin, nullptr, nullptr, dw, nullptr);
   SG_CHECK_LAUNCH();
   return SG_OK;
 }

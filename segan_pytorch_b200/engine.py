@@ -7,6 +7,7 @@ Layer geometry follows the reference (file:line into santi-pdp/segan_pytorch):
   encoder block  = reflect-pad(14,15) -> Conv1d(k31,s4) -> [BatchNorm1d] -> PReLU   segan/models/modules.py:91-105
   decoder block  = ConvTranspose1d(k31,s4,p13)[:-1] -> PReLU | Tanh                 segan/models/modules.py:135-141
   G wiring       = 5 enc -> cat(z, h) -> 5 x (cat(h, alpha*skip), dec)              segan/models/generator.py:180-230
+                   (no_z: h alone into dec 0; skip=False: every dec block reads h alone)
   D wiring       = 5 x (phase shift, enc with BN) -> FC 16384-256-128-1             segan/models/discriminator.py:150-194
 
 HBM layouts are described in include/segan_b200.h and DESIGN.md.
@@ -844,10 +845,14 @@ class GeneratorEngine(_NetEngine):
         self.fmaps = list(m.enc_fmaps)
         self.nl = len(self.fmaps)
         self.enc_bias = m.bias
-        self.sum_merge = getattr(m, "skip_merge", "concat") == "sum"
+        # topology: z channels ahead of the code in decoder block 0 (0 with no_z) and whether the decoder merges
+        # skips at all (skip=False: every decoder block and the waveform end read the previous block alone)
+        self.zc = 0 if getattr(m, "no_z", False) else m.z_dim
+        self.has_skip = getattr(m, "skip", True)
+        self.sum_merge = self.has_skip and getattr(m, "skip_merge", "concat") == "sum"
         # skip_type='conv': the skip of encoder level l is Conv1d(C, C, K)(a[l]) (weights alpha_l.skip_k.weight /
         # .bias, small region of the bucket) and has no alpha -- every alpha use below reads 1
-        self.conv_skip = getattr(m, "skip_type", "alpha") == "conv"
+        self.conv_skip = self.has_skip and getattr(m, "skip_type", "alpha") == "conv"
         self.skip_kw = getattr(m, "skip_kwidth", 11)
         self.packed = {}
 
@@ -861,8 +866,8 @@ class GeneratorEngine(_NetEngine):
         for l in range(nl - 1):
             ls.append(PackedLayer("dec_blocks.%d.deconv.weight" % l, 1, self.dec_cout(l), self.dec_cin(l), 0,
                                   "Wt%d" % l, "Wtd%d" % l,
-                                  alpha_name=(("alpha_%d.skip_k" % (nl - 1 - l)) if l > 0 and not self.conv_skip
-                                              else None),
+                                  alpha_name=(("alpha_%d.skip_k" % (nl - 1 - l))
+                                              if l > 0 and self.has_skip and not self.conv_skip else None),
                                   tied=(self.sum_merge and l > 0)))
         ls += [PackedLayer("enc_blocks.%d.conv.weight" % l, 0, fm[l], fm[l - 1], 0, "Wf%d" % l, "Wdg%d" % l)
                for l in range(nl - 1, 0, -1)]
@@ -882,10 +887,10 @@ class GeneratorEngine(_NetEngine):
         if self.sum_merge:                       # tied halves: W (hi + alpha skip) = [W | alpha W] cat(hi, skip)
             w = torch.cat((w, w), 0)
         self.packed["w_last_dup"] = w.reshape(w.shape[0], 1, KW).contiguous()
-        alpha = self.alpha_for_dec(l)
-        half = w.shape[0] // 2
         weff = w.clone()
-        weff[half:] = weff[half:] * alpha.view(-1, 1)
+        if self.has_skip:
+            half = w.shape[0] // 2
+            weff[half:] = weff[half:] * self.alpha_for_dec(l).view(-1, 1)
         self.packed["w_last_eff"] = weff.contiguous()
         # tensor-core route of the waveform-end layers: single-tap operands (tiny tensors, torch ops)
         wcol = wave_col_weights(self.pview("enc_blocks.0.conv.weight"), dev)
@@ -928,16 +933,19 @@ class GeneratorEngine(_NetEngine):
         self._alpha_fixed = True
 
     def dec_cin(self, l):
-        """Input channels of decoder block l AS THE GEMM SEES THEM: cat(z, code) for block 0, cat(decoder, skip)
-        afterwards -- also with skip_merge='sum', which runs as the concat GEMM with tied weight halves."""
-        return 2 * self.fmaps[-1] if l == 0 else 2 * self.fmaps[self.nl - 1 - l]
+        """Input channels of decoder block l AS THE GEMM SEES THEM: cat(z, code) (the code alone with no_z) for
+        block 0, cat(decoder, skip) afterwards -- also with skip_merge='sum', which runs as the concat GEMM with
+        tied weight halves -- or the decoder output alone without skips."""
+        if l == 0:
+            return self.zc + self.fmaps[-1]
+        return (2 if self.has_skip else 1) * self.fmaps[self.nl - 1 - l]
 
     def dec_cout(self, l):
         return self.fmaps[self.nl - 2 - l] if l < self.nl - 1 else 1
 
     def alpha_for_dec(self, l):
-        """alpha of the skip merged before decoder block l (None for block 0: cat(z, h))."""
-        if l == 0:
+        """alpha of the skip merged before decoder block l (None for block 0: cat(z, h), and without skips)."""
+        if l == 0 or not self.has_skip:
             return None
         if self.conv_skip:                       # the skip conv's output is merged unscaled
             c, key = self.fmaps[self.nl - 1 - l], "g.ones%d" % self.fmaps[self.nl - 1 - l]
@@ -1023,23 +1031,27 @@ class GeneratorEngine(_NetEngine):
                 hpb[l], ab[l] = hp[l], a[l]
             if self.conv_skip and l < nl - 1:
                 sk[l], skb[l] = self._skip_conv_fwd(l, a[l], B, Lq[l], buf, twins, alias)
-        # ---- z
-        zc = z.shape[1]
-        z16 = buf.get("g.z16", (B, Lq[-1], zc), F16, dev)
-        zf = z.contiguous().float()
-        _lib.call("sg_ncl_to_nlc", _p(zf), B, zc, Lq[-1], _p(z16), SG_F16, st)
-        if twins:
-            z16b = buf.get("g.z16b", (B, Lq[-1], zc), GT, dev)
-            _lib.call("sg_ncl_to_nlc", _p(zf), B, zc, Lq[-1], _p(z16b), GS, st)
-        elif alias:
-            z16b = z16
+        # ---- z (none with no_z: decoder block 0 reads the code alone)
+        z16 = None
+        if self.zc:
+            zc = z.shape[1]
+            assert zc == self.zc, "z has %d channels, the Generator was built with z_dim %d" % (zc, self.zc)
+            z16 = buf.get("g.z16", (B, Lq[-1], zc), F16, dev)
+            zf = z.contiguous().float()
+            _lib.call("sg_ncl_to_nlc", _p(zf), B, zc, Lq[-1], _p(z16), SG_F16, st)
+            if twins:
+                z16b = buf.get("g.z16b", (B, Lq[-1], zc), GT, dev)
+                _lib.call("sg_ncl_to_nlc", _p(zf), B, zc, Lq[-1], _p(z16b), GS, st)
+            elif alias:
+                z16b = z16
         # ---- decoder
         ad, dd = [None] * nl, [None] * nl
-        src0, src1 = z16, hp[nl - 1]
+        src0, src1 = (z16, hp[nl - 1]) if self.zc else (hp[nl - 1], None)
         lin = Lq[-1]
         for l in range(nl - 1):
             cin, cout = self.dec_cin(l), self.dec_cout(l)
-            assert src0.shape[-1] + src1.shape[-1] == cin
+            c1 = 0 if src1 is None else src1.shape[-1]
+            assert src0.shape[-1] + c1 == cin
             dd[l] = buf.get("g.dd%d" % l, (B, 4 * lin, cout), F16, dev)
             slope = self.pview("dec_blocks.%d.act.weight" % l)
             fz = fused(lin, 0)
@@ -1056,7 +1068,7 @@ class GeneratorEngine(_NetEngine):
             run_f(src0, src1, lin, 0, SG_F16, self.packed["Wt%d" % l], SG_F16, cin, 4 * cout,
                   tap_ranges("deconv_fwd", cout, cin, 4 * cout), dst, SG_F16, lin, 0, 0, lin, B,
                   bias=self.pview("dec_blocks.%d.deconv.bias" % l), bias_mod=cout,
-                  a0_c=src0.shape[-1], a1_c=src1.shape[-1], backend=self.backend, **fkw)
+                  a0_c=src0.shape[-1], a1_c=c1, backend=self.backend, **fkw)
             if twins:
                 ddb[l] = buf.get("g.ddb%d" % l, (B, 4 * lin, cout), GT, dev)
             if not fz:
@@ -1065,17 +1077,22 @@ class GeneratorEngine(_NetEngine):
             if alias:
                 ddb[l] = dd[l]
             lin *= 4
-            src0, src1 = dd[l], (sk if self.conv_skip else a)[nl - 2 - l]
+            src0 = dd[l]
+            src1 = (sk if self.conv_skip else a)[nl - 2 - l] if self.has_skip else None
         y = torch.empty(B, 1, L, dtype=F32, device=dev)
         blast = self.pview("dec_blocks.%d.deconv.bias" % (nl - 1))
         if wave_on_tensor_cores():
-            cl = src0.shape[-1] + src1.shape[-1]
+            c1 = 0 if src1 is None else src1.shape[-1]
+            cl = src0.shape[-1] + c1
             P = buf.get("g.P", (B, lin, 64), F32, dev)
             run_f(src0, src1, lin, 0, SG_F16, self.packed["W2_last"], SG_F16, cl, 64, tap_ranges("full", 0, cl, 64),
-                  P, SG_F32, lin, 0, 0, lin, B, d_lo=0, d_hi=0, w_tap0=4, a0_c=src0.shape[-1], a1_c=src1.shape[-1],
+                  P, SG_F32, lin, 0, 0, lin, B, d_lo=0, d_hi=0, w_tap0=4, a0_c=src0.shape[-1], a1_c=c1,
                   backend=self.backend)
             _lib.call("sg_wave_shiftadd_tanh", _p(P), B, lin, _p(blast), _p(y), st)
         else:
+            if not self.has_skip:
+                raise NotImplementedError("a Generator without skips (skip=False) needs the tensor-core waveform "
+                                          "route (SEGAN_B200_WAVE=tc)")
             _lib.call("sg_wave_deconv_fwd", _p(src0), src0.shape[-1], _p(src1), src1.shape[-1], B, lin,
                       _p(self.packed["w_last_eff"]), _p(blast), _p(y), st)
         self.packs_consumed()
@@ -1112,11 +1129,12 @@ class GeneratorEngine(_NetEngine):
             _lib.call("sg_nlc_to_ncl", _p(t16), SG_F16, B, C_, L_, _p(out), st)
             return out
         want = (lambda k: True) if only is None else (lambda k: k in only)
+        want_zc = self.zc > 0 and want("enc_zc")          # no_z: the reference's hall has no enc_zc
         for l in range(nl):
-            if want("enc_%d" % l) or (l == nl - 1 and want("enc_zc")):
+            if want("enc_%d" % l) or (l == nl - 1 and want_zc):
                 a = to_ncl(ctx["a"][l], self.fmaps[l], Lq[l])
                 hall["enc_%d" % l] = torch.nn.functional.prelu(a, self.pview("enc_blocks.%d.act.weight" % l))
-        if want("enc_zc"):
+        if want_zc:
             zc = ctx["z16"].shape[-1]
             hall["enc_zc"] = torch.cat((to_ncl(ctx["z16"], zc, Lq[-1]), hall["enc_%d" % (nl - 1)]), 1)
         lin = Lq[-1]
@@ -1172,20 +1190,32 @@ class GeneratorEngine(_NetEngine):
             # dW'[n=(s,k)][kc=(src,s',c)] over position pairs; the s == s' blocks are the gradient: folded (and
             # cleared for the next step) by sg_last_deconv_wgrad_fold into dW (alpha on the skip half) and dalpha
             dwq = buf.get("g.dwq_last", (128 * 2 * cin,), F32, dev)
-            a_train = not self.conv_skip and self._param("alpha_0.skip_k").requires_grad
-            with on_side(side):
-                run_w(colg, lin // 2, GS, ctx["ddb"][l - 1], ctx["skb"][0], lin // 2, 0, GS, 2 * cin, 128,
-                      tap_ranges("full", 0, 2 * cin, 128), dwq, B, d_lo=0, d_hi=0, dw_tap0=4, ksplit=74,
-                      a0_c=cin, a1_c=cin, backend=self.backend)
-                gw_dst = self.gview("dec_blocks.%d.deconv.weight" % l)
-                if self.sum_merge:
-                    gw_dst = buf.get("g.gw_last2", (cin, 1, KW), F32, dev, zero=True)
-                _lib.call("sg_last_deconv_wgrad_fold", _p(dwq), half, _p(self.packed["w_last_dup"]),
-                          _p(self.alpha_for_dec(l)), _p(gw_dst),
-                          _p(self.gview("alpha_0.skip_k").view(-1)) if a_train else None, _stream())
-                if self.sum_merge:
-                    self.gview("dec_blocks.%d.deconv.weight" % l).add_(gw_dst[:half] + gw_dst[half:])
+            if not self.has_skip:
+                # one source: kc = (s', c) over the decoder output alone, folded without alpha
+                with on_side(side):
+                    run_w(colg, lin // 2, GS, ctx["ddb"][l - 1], None, lin // 2, 0, GS, 2 * cin, 128,
+                          tap_ranges("full", 0, 2 * cin, 128), dwq, B, d_lo=0, d_hi=0, dw_tap0=4, ksplit=74,
+                          a0_c=2 * cin, backend=self.backend)
+                    _lib.call("sg_last_deconv_wgrad_fold_1src", _p(dwq), cin,
+                              _p(self.gview("dec_blocks.%d.deconv.weight" % l)), _stream())
+            else:
+                a_train = not self.conv_skip and self._param("alpha_0.skip_k").requires_grad
+                with on_side(side):
+                    run_w(colg, lin // 2, GS, ctx["ddb"][l - 1], ctx["skb"][0], lin // 2, 0, GS, 2 * cin, 128,
+                          tap_ranges("full", 0, 2 * cin, 128), dwq, B, d_lo=0, d_hi=0, dw_tap0=4, ksplit=74,
+                          a0_c=cin, a1_c=cin, backend=self.backend)
+                    gw_dst = self.gview("dec_blocks.%d.deconv.weight" % l)
+                    if self.sum_merge:
+                        gw_dst = buf.get("g.gw_last2", (cin, 1, KW), F32, dev, zero=True)
+                    _lib.call("sg_last_deconv_wgrad_fold", _p(dwq), half, _p(self.packed["w_last_dup"]),
+                              _p(self.alpha_for_dec(l)), _p(gw_dst),
+                              _p(self.gview("alpha_0.skip_k").view(-1)) if a_train else None, _stream())
+                    if self.sum_merge:
+                        self.gview("dec_blocks.%d.deconv.weight" % l).add_(gw_dst[:half] + gw_dst[half:])
         else:
+            if not self.has_skip:
+                raise NotImplementedError("a Generator without skips (skip=False) needs the tensor-core waveform "
+                                          "route (SEGAN_B200_WAVE=tc)")
             if self.conv_skip:
                 raise NotImplementedError("skip_type='conv' needs the tensor-core waveform route (SEGAN_B200_WAVE=tc)")
             dweff = buf.get("g.dweff", (cin, KW), F32, dev, zero=True)
@@ -1213,10 +1243,10 @@ class GeneratorEngine(_NetEngine):
             _lib.call("sg_stat_grads", _p(red), cout, 3, _p(self.gview("dec_blocks.%d.act.weight" % l)),
                       _p(self.gview("dec_blocks.%d.deconv.bias" % l)), None, st)
             if l == 0:
-                s0, s1 = ctx["z16b"], ctx["hpb"][nl - 1]
+                s0, s1 = (ctx["z16b"], ctx["hpb"][nl - 1]) if self.zc else (ctx["hpb"][nl - 1], None)
             else:
-                s0, s1 = ctx["ddb"][l - 1], ctx["skb"][nl - 1 - l]
-            c0, c1 = s0.shape[-1], s1.shape[-1]
+                s0, s1 = ctx["ddb"][l - 1], (ctx["skb"][nl - 1 - l] if self.has_skip else None)
+            c0, c1 = s0.shape[-1], (0 if s1 is None else s1.shape[-1])
             taps = tap_ranges("deconv_fwd", cout, cin, 4 * cout)
             dwp = self.mgrad(self.by_name["dec_blocks.%d.deconv.weight" % l])     # packed gradient slot (dWeff)
             with on_side(side):
@@ -1226,7 +1256,8 @@ class GeneratorEngine(_NetEngine):
                       backend=self.backend)
                 if l == 0 and reducer is not None:
                     reducer.ready(0, launch=True)              # every decoder weight gradient has been enqueued
-            # data gradient w.r.t. cat(s0, s1); block 0 only needs the encoder half (z gets no gradient)
+            # data gradient w.r.t. cat(s0, s1); block 0 only needs the code's columns [zc, zc + C) (z gets no
+            # gradient)
             if self.conv_skip and l > 0:
                 g_in = buf.get("g.gin%d" % l, (B, lin, cin // 2), GT, dev)
                 for dst, n0 in ((g_in, 0), (buf.get("g.gsk%d" % (nl - 1 - l), (B, lin, cin // 2), GT, dev), cin // 2)):
@@ -1237,7 +1268,7 @@ class GeneratorEngine(_NetEngine):
                 g_in = buf.get("g.gin%d" % l, (B, lin, cin), GT, dev)
                 run_f(g_ad, None, lin, 0, GS, self.packed["Wtd%d" % l], GS, 4 * cout, cin,
                       tap_ranges("deconv_dgrad", cout, 4 * cout, cin), g_in, GS, lin, 0, 0, lin, B,
-                      n_lo=(cin // 2 if l == 0 else 0), n_hi=cin, backend=self.backend)
+                      n_lo=(self.zc if l == 0 else 0), n_hi=cin, backend=self.backend)
             g_next = g_in
         # ---- encoder blocks nl-1 .. 0
         g_hp = None
@@ -1247,12 +1278,14 @@ class GeneratorEngine(_NetEngine):
             red = red_enc[l]
             slope = self.pview("enc_blocks.%d.act.weight" % l)
             if l == nl - 1:
-                gin0 = buf.t["g.gin0"]
-                gh_ptr = C.c_void_p(gin0.data_ptr() + 2 * (gin0.shape[-1] // 2))
+                gin0 = buf.t["g.gin0"]                  # [B][Lq][zc + C]: the code's gradient from column zc
+                gh_ptr = C.c_void_p(gin0.data_ptr() + 2 * self.zc)
                 _lib.call("sg_act_bwd_reduce", gh_ptr, gin0.shape[-1], 0, 0, None, None, 0, _p(a[l]), SG_F16, B, Lq[l],
                           cout, None, None, _p(slope), ACT_PRELU, _p(red), _p(g_a), st)
             else:
-                if self.conv_skip:
+                if not self.has_skip:
+                    gadd_ptr, gadd_ld = None, 0
+                elif self.conv_skip:
                     gadd_ptr, gadd_ld = _p(self._skip_conv_bwd(l, ctx, side)), cout
                 else:
                     gsk = buf.t["g.gin%d" % (nl - 1 - l)]

@@ -1,7 +1,8 @@
 """Drop-in `Generator` (reference: segan/models/generator.py:18-230).
 
 Same constructor signature, same `forward(x, z=None, ret_hid=False)` contract, same state-dict
-keys; the arithmetic runs in libsegan_b200.so (segan_pytorch_b200.engine.GeneratorEngine)."""
+keys; the arithmetic runs in libsegan_b200.so (segan_pytorch_b200.engine.GeneratorEngine).  Served: alpha / constant /
+conv skips with concat or sum merge, skip=False, no_z=True and any z_dim that is a positive multiple of 64."""
 import torch
 import torch.nn as nn
 
@@ -135,17 +136,26 @@ class Generator(Model):
         self.enc_fmaps = list(fmaps)
         self.skip_merge = skip_merge
         self.skip_type, self.skip_kwidth = skip_type, skip_kwidth
-        self._served = (ninputs == 1 and skip and not no_z and skip_merge in ('concat', 'sum')
-                        and (skip_type in ('alpha', 'constant')
-                             or (skip_type == 'conv' and _engine.skipconv_served(skip_kwidth)))
+        # no_z / skip=False / z_dim only change the channel counts the decoder's GEMMs contract over; z must be a
+        # whole number of 64-channel K blocks so that the z / code split of block 0 falls on a block boundary
+        self._served = (ninputs == 1 and (not skip or (skip_merge in ('concat', 'sum')
+                                                       and (skip_type in ('alpha', 'constant')
+                                                            or (skip_type == 'conv'
+                                                                and _engine.skipconv_served(skip_kwidth)))))
                         and norm_type is None
                         and all(k == 31 for k in kwidth) and all(k == 31 for k in dec_kwidth)
                         and all(p == 4 for p in poolings) and all(p == 4 for p in dec_poolings)
                         and list(dec_fmaps) == fmaps[::-1][1:] + [1]
-                        and (self.z_dim if self.z_dim is not None else fmaps[-1]) == fmaps[-1]
                         and all(f % 64 == 0 for f in fmaps) and fmaps[0] == 64)
+        self._unserved = None if self._served else ("this Generator configuration is outside the built hot path "
+                                                     "(SEGAN+ layout: k=31, stride 4, no norm, fmaps 64..)")
         if self.z_dim is None and not no_z:
             self.z_dim = fmaps[-1]
+        if self._served and not no_z and not (isinstance(self.z_dim, int) and self.z_dim > 0 and self.z_dim % 64 == 0):
+            self._served = False
+            self._unserved = ("z_dim=%r is not served: it must be a positive multiple of 64, so that the split "
+                              "between z and the code in decoder block 0 falls on a 64-channel K block of the "
+                              "tensor-core GEMM" % (self.z_dim,))
         self.z_device = 'cpu'   # 'cpu' = draw z on the CPU generator like generator.py:197-199; 'cuda' = on device
         self._engine = None
 
@@ -153,8 +163,7 @@ class Generator(Model):
     @property
     def engine(self):
         if not self._served:
-            raise NotImplementedError("this Generator configuration is outside the built hot path "
-                                      "(SEGAN+ defaults: alpha skips, concat merge, k=31, stride 4, no norm)")
+            raise NotImplementedError(self._unserved)
         if self._engine is None:
             self._engine = _engine.GeneratorEngine(self)
         return self._engine
@@ -175,16 +184,19 @@ class Generator(Model):
         eng = self.engine
         _engine._require_cuda(x)
         B, _, L = x.shape
-        if z is None:
-            code_len = L // (4 ** len(self.enc_blocks))
-            if self.z_device == 'cpu':
-                z = torch.randn(B, self.z_dim, code_len).to(x.device)      # generator.py:197-199
-            else:
-                z = torch.randn(B, self.z_dim, code_len, device=x.device)
-        if len(z.size()) != 3:
-            raise ValueError('len(z.size) {} != len(hi.size) {}'.format(len(z.size()), 3))
-        if not hasattr(self, 'z'):
-            self.z = z                                                   # generator.py:203-204
+        if self.no_z:
+            z = None                     # generator.py:193-208: a passed z is ignored, none is drawn, self.z never set
+        else:
+            if z is None:
+                code_len = L // (4 ** len(self.enc_blocks))
+                if self.z_device == 'cpu':
+                    z = torch.randn(B, self.z_dim, code_len).to(x.device)      # generator.py:197-199
+                else:
+                    z = torch.randn(B, self.z_dim, code_len, device=x.device)
+            if len(z.size()) != 3:
+                raise ValueError('len(z.size) {} != len(hi.size) {}'.format(len(z.size()), 3))
+            if not hasattr(self, 'z'):
+                self.z = z                                                   # generator.py:203-204
         eng.bind()
         if torch.is_grad_enabled() and any(p.requires_grad for p in super().parameters()):
             params = [p for _, p in self.named_parameters()]

@@ -199,6 +199,9 @@ DP_OVERLAP = os.environ.get("SEGAN_B200_DP_OVERLAP", "1").lower() not in ("0", "
 # the replays following the first one were seen to hang (NCCL 2.28.9, eager collectives -- barriers -- mixed with
 # the captured ones).  Default: three graphs with one eager all-reduce per bucket between them.
 DP_CAPTURE = os.environ.get("SEGAN_B200_DP_CAPTURE", "0").lower() not in ("0", "off", "no", "false")
+# SEGAN's regression term (--reg_loss, model.py:79,318) -> its fused loss + gradient kernel.  WSEGAN's denoising term
+# is always L1 (model.py:663).
+REG_LOSS_KERNELS = {'l1_loss': 'sg_l1_loss_bwd', 'mse_loss': 'sg_mse_loss_bwd'}
 
 
 class GradReducer(object):
@@ -276,7 +279,9 @@ class SEGAN(Model):
         flat = inwav[0, 0].to(dev)
         x.view(-1)[:T].copy_(flat)
         code_len = N // (4 ** len(self.G.enc_blocks))
-        if z is None:
+        if self.G.no_z:
+            zb = None                                      # generator.py:193-208: no z drawn, G.z never set
+        elif z is None:
             z0 = torch.randn(1, self.G.z_dim, code_len).to(dev)
             if not hasattr(self.G, 'z'):
                 self.G.z = z0
@@ -286,7 +291,8 @@ class SEGAN(Model):
             if not hasattr(self.G, 'z'):
                 self.G.z = z0
             zrest = z0
-        zb = torch.cat([z0[:1]] + [zrest[:1]] * (nchunks - 1), 0) if nchunks > 1 else z0[:1]
+        if not self.G.no_z:
+            zb = torch.cat([z0[:1]] + [zrest[:1]] * (nchunks - 1), 0) if nchunks > 1 else z0[:1]
         last = 'enc_{}'.format(len(self.G.enc_blocks) - 1)
         with torch.no_grad():
             y, hall = self.G(x, z=zb, ret_hid=(last,))     # only the code of model.py:149 is converted to NCL
@@ -384,7 +390,7 @@ class SEGAN(Model):
         N = 16384
         dev = next(super(Model, self.G).parameters()).device
         code_len = N // (4 ** len(self.G.enc_blocks))
-        zdim = self.G.z_dim
+        zdim = None if self.G.no_z else self.G.z_dim
         group_windows = int(group_windows or 2 * batch)
         coef = float(self.preemph)
         os.makedirs(out_dir, exist_ok=True)
@@ -415,10 +421,11 @@ class SEGAN(Model):
                         first.append(w0)
                         files.append((path, w0, T))
                         w0 += n
-                    # one fresh z per file, drawn in file order from torch's CPU generator (generator.py:197-199)
-                    zf = torch.randn(len(files), zdim, code_len)
+                    # one fresh z per file, drawn in file order from torch's CPU generator (generator.py:197-199);
+                    # none with no_z
+                    zf = torch.randn(len(files), zdim, code_len).pin_memory() if zdim is not None else None
                     q_in.put(dict(pcm=pcm, prev=prev.pin_memory(), valid=valid.pin_memory(), files=files,
-                                  first=torch.tensor(first, dtype=torch.long), zf=zf.pin_memory(), nwin=nwin))
+                                  first=torch.tensor(first, dtype=torch.long), zf=zf, nwin=nwin))
                     group, nwin = [], 0
                 for path in wav_paths:
                     rate, wav = wavfile.read(path)
@@ -468,7 +475,8 @@ class SEGAN(Model):
 
         def upload(g):
             with torch.cuda.stream(h2d):
-                d = {k: g[k].to(dev, non_blocking=True) for k in ('pcm', 'prev', 'valid', 'zf')}
+                d = {k: (g[k].to(dev, non_blocking=True) if g[k] is not None else None)
+                     for k in ('pcm', 'prev', 'valid', 'zf')}
                 d['ready'] = torch.cuda.Event()
                 d['ready'].record(h2d)
             return d
@@ -482,17 +490,19 @@ class SEGAN(Model):
             nw = g['nwin']
             x = torch.empty(nw, 1, N, dtype=torch.float32, device=dev)
             _lib.call("sg_pcm16_to_wave", _p(d['pcm']), _p(d['prev']), nw, N, coef, _p(x), _p(d['valid']), _stream())
-            if not hasattr(self.G, 'z'):
+            if zdim is not None and not hasattr(self.G, 'z'):
                 self.G.z = d['zf'][:1].clone()             # generator.py:203-204: the first z ever
             first = g['first'].to(dev)
             y = torch.empty(nw, N, dtype=torch.float32, device=dev)
             with torch.no_grad():
                 for b0 in range(0, nw, batch):
                     b1 = min(nw, b0 + batch)
-                    zb = self.G.z[:1].expand(b1 - b0, -1, -1).clone()
-                    sel = (first >= b0) & (first < b1)
-                    if bool(sel.any()):
-                        zb[first[sel] - b0] = d['zf'][sel]
+                    zb = None
+                    if zdim is not None:
+                        zb = self.G.z[:1].expand(b1 - b0, -1, -1).clone()
+                        sel = (first >= b0) & (first < b1)
+                        if bool(sel.any()):
+                            zb[first[sel] - b0] = d['zf'][sel]
                     y[b0:b1] = self.G(x[b0:b1], z=zb).view(b1 - b0, N)
             out = torch.empty_like(y)
             if coef > 0:
@@ -503,7 +513,8 @@ class SEGAN(Model):
             done = torch.cuda.Event()
             done.record(main)
             for t_ in (d['pcm'], d['prev'], d['valid'], d['zf']):
-                t_.record_stream(main)
+                if t_ is not None:
+                    t_.record_stream(main)
             host = torch.empty(nw * N, dtype=torch.float32).pin_memory()
             with torch.cuda.stream(d2h):
                 d2h.wait_event(done)
@@ -552,6 +563,8 @@ class SEGAN(Model):
     # one LSGAN + L1 step (model.py:283-321) on device-resident (B,1,L) tensors
     # ------------------------------------------------------------------------------------------
     def _sample_z(self, B, code_len, dev):
+        if self.G.no_z:
+            return None                  # the reference draws no z (and consumes no random numbers) with no_z
         if self.z_device == 'cpu':
             z = torch.randn(B, self.G.z_dim, code_len).to(dev)        # generator.py:197-199
         else:
@@ -594,13 +607,17 @@ class SEGAN(Model):
         B, _, L = clean.shape
         dev = clean.device
         nl = len(self.D.enc_blocks)
-        if self.reg_loss_name != 'l1_loss':
-            raise NotImplementedError("reg_loss %r: only 'l1_loss' (train.py:179 default) is built" % self.reg_loss_name)
+        if self.reg_loss_name not in REG_LOSS_KERNELS:
+            raise NotImplementedError("reg_loss %r is not built: the G regression term runs as a fused kernel for %s"
+                                      % (self.reg_loss_name, " / ".join(repr(k) for k in REG_LOSS_KERNELS)))
         if shifts3 is None:        # python `random` draw order of the reference: real, fake, G-step pass
             shifts3 = [draw_phase_shifts(nl, self.D.phase_shift) for _ in range(3)]
-        if z is None and self.z_device == 'cpu':
+        if self.G.no_z:
+            z = None
+        elif z is None and self.z_device == 'cpu':
             z = self._sample_z(B, L // (4 ** len(self.G.enc_blocks)), dev)
-        st = self._graph_state(clean, noisy, Gopt, Dopt, l1_weight, z is None)
+        sample_z = z is None and not self.G.no_z          # z drawn on the device inside the step
+        st = self._graph_state(clean, noisy, Gopt, Dopt, l1_weight, sample_z)
         if st is None:
             # ---- eager schedule
             if losses is None:
@@ -634,7 +651,7 @@ class SEGAN(Model):
         st.ring_ev[i] = torch.cuda.Event()
         st.ring_ev[i].record()
         if st.graphs is None:
-            self._capture_step(st, z is None, shifts3, l1_weight, Gopt, Dopt)
+            self._capture_step(st, sample_z, shifts3, l1_weight, Gopt, Dopt)
         else:
             # parameters touched outside the step (checkpoint load ...): import them; D's operands of graph 1 were
             # emitted by the previous replay of graph 2, so they are refreshed here
@@ -707,8 +724,9 @@ class SEGAN(Model):
         _, c = de.forward(Genh, noisy, shifts3[2], training=True, twins=False, shifts_dev=sdev)   # no weight gradients here
         gy = ge.buf.get("g.gy", (B, 1, L), torch.float32, dev, zero=True)
         de.backward(c, 1.0, 1.0, param_grads=False, input_grad=gy, loss_out=lptr(2))
-        _lib.call("sg_l1_loss_bwd", _p(Genh), _p(clean.contiguous()), B * L, float(l1_weight), lptr(3), _p(gy), 1,
-                  float(_engine.LOSS_SCALE), _stream())
+        # model.py:318: l1_weight * reg_loss(Genh, clean) -- logged as g_l1 whatever reg_loss is
+        _lib.call(REG_LOSS_KERNELS[self.reg_loss_name], _p(Genh), _p(clean.contiguous()), B * L, float(l1_weight),
+                  lptr(3), _p(gy), 1, float(_engine.LOSS_SCALE), _stream())
         ge.backward(gctx, gy, reducer=reducer)
 
     # -- CUDA graphs ------------------------------------------------------------------------------
@@ -743,7 +761,8 @@ class SEGAN(Model):
             nl = len(self.D.enc_blocks)
             st.clean = torch.empty_like(clean)
             st.noisy = torch.empty_like(noisy)
-            st.z = torch.empty(B, self.G.z_dim, L // (4 ** len(self.G.enc_blocks)), device=dev)
+            st.z = (None if self.G.no_z else
+                    torch.empty(B, self.G.z_dim, L // (4 ** len(self.G.enc_blocks)), device=dev))
             st.losses = torch.zeros(4, dtype=torch.float32, device=dev)
             st.shifts = torch.zeros(3 * nl, dtype=torch.int32, device=dev)
             st.ring = torch.zeros(32, 3 * nl, dtype=torch.int32).pin_memory()
@@ -995,7 +1014,9 @@ class WSEGAN(SEGAN):
         nsh = iter(shifts) if shifts is not None else None
         draw = (lambda: next(nsh)) if nsh is not None else (lambda: draw_phase_shifts(nl, self.D.phase_shift))
         sh = [draw()]                                                      # D(real)
-        sample_z = z is None and self.z_device != 'cpu'
+        if self.G.no_z:
+            z = None
+        sample_z = z is None and self.z_device != 'cpu' and not self.G.no_z
         if z is None and not sample_z:
             z = self._sample_z(B, L // (4 ** len(self.G.enc_blocks)), dev)
         sh.append(draw())                                                  # D(fake)
@@ -1160,7 +1181,8 @@ class WSEGAN(SEGAN):
             ntab = n_pass * nl + (B if self.misalign_pair else 0)
             st.clean = torch.empty_like(clean)
             st.noisy = torch.empty_like(noisy)
-            st.z = torch.empty(B, self.G.z_dim, L // (4 ** len(self.G.enc_blocks)), device=dev)
+            st.z = (None if self.G.no_z else
+                    torch.empty(B, self.G.z_dim, L // (4 ** len(self.G.enc_blocks)), device=dev))
             st.losses = torch.zeros(4, dtype=torch.float32, device=dev)
             st.table = torch.zeros(ntab, dtype=torch.int32, device=dev)     # phase shifts of every pass [+ permutation]
             st.interf = torch.zeros_like(clean) if self.interf_pair else None
