@@ -404,6 +404,18 @@ int sg_snorm_grad(float* dwp, const float* master, int n_taps, int nc, int kc, c
 int sg_snorm_coef(const double* red, const float* bias, int C, const float* scal, float* coef_out, void* stream);
 int sg_snorm_rank1(float* dwp, int n_taps, int nc, int kc, int n_pass, const float* u, const float* v,
                    const float* coef, void* stream);
+/* Row-strided variants (the Generator's tensors): the matrix is M[n_taps][nc][kc] with rows `ld` floats apart.
+ *   ld > kc serves a tied skip_merge='sum' master [W | W]: the iteration sees one half W, and the correction is
+ *   applied to n_copies halves at column offsets 0, kc, 2 kc ...
+ *   A decoder master M[9][4 Cout][Cin] is the same bytes as [36][Cout][Cin] (tap t = 4 (d + 4) + r), so n_taps = 36,
+ *   nc = Cout, kc = Cin is exactly torch's spectral_norm(dim = 1) of ConvTranspose1d's W[Cin][Cout][31]: u per output
+ *   channel, v per (tap, input channel); the structural-zero taps keep v = 0.
+ *   sg_snorm_sigma_ld reduces in a fixed order (no float atomics): the same master and vectors give the same bits
+ *   on every run and rank.  work: nc + n_taps * ceil(kc / 256) floats. */
+int sg_snorm_sigma_ld(const float* master, int n_taps, int nc, int kc, int ld, float* u, float* v, float* scal,
+                      float* work, int training, void* stream);
+int sg_snorm_rank1_ld(float* dwp, int n_taps, int nc, int kc, int ld, int n_copies, int n_pass, const float* u,
+                      const float* v, const float* coef, void* stream);
 int sg_wave_wgrad_fold(float* dwq /* the blocks read are cleared */, int cin, float* dw, void* stream);
 int sg_last_deconv_wgrad_fold(float* dwq /* the blocks read are cleared */, int half, const float* w, const float* alpha, float* dw,
                               float* dalpha, void* stream);

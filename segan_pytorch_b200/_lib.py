@@ -84,6 +84,8 @@ _SIGS = {
     "sg_snorm_grad": [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp],
     "sg_snorm_coef": [_vp, _vp, _i, _vp, _vp, _vp],
     "sg_snorm_rank1": [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp],
+    "sg_snorm_sigma_ld": [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _vp],
+    "sg_snorm_rank1_ld": [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp],
     "sg_alpha_grad": [_vp, _vp, _i, _i, _i, _vp, _i, _vp, _vp],
     "sg_wave_wgrad_fold": [_vp, _i, _vp, _vp],
     "sg_last_deconv_wgrad_fold": [_vp, _i, _vp, _vp, _vp, _vp, _vp],

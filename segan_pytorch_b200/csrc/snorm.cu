@@ -122,10 +122,11 @@ __global__ void snorm_coef_kernel(const double* __restrict__ red, const float* _
   if (threadIdx.x == 0) *coef = (float)(sh[0] * (double)scal[3]);
 }
 
-// dwp[t][n][k] -= sum_p coef[p] * u[p][n] * v[p][t][k]     (the sigma terms of P passes, one sweep)
+// dwp[t][n][c * kc + k] -= sum_p coef[p] * u[p][n] * v[p][t][k]  for every copy c < n_copies, rows of ld floats
+// (the sigma terms of P passes, one sweep; ld = kc and one copy: the plain packed layout)
 __global__ void __launch_bounds__(256)
-snorm_rank1_kernel(float* __restrict__ dwp, int T, int nc, int kc, int P, const float* __restrict__ u,
-                   const float* __restrict__ v, const float* __restrict__ coef) {
+snorm_rank1_kernel(float* __restrict__ dwp, int T, int nc, int kc, int ld, int n_copies, int P,
+                   const float* __restrict__ u, const float* __restrict__ v, const float* __restrict__ coef) {
   const int64_t total = (int64_t)T * nc * kc;
   const int64_t vstride = (int64_t)T * kc;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
@@ -134,8 +135,68 @@ snorm_rank1_kernel(float* __restrict__ dwp, int T, int nc, int kc, int P, const 
     const int n = (int)(r % nc), t = (int)(r / nc);
     float corr = 0.f;
     for (int p = 0; p < P; ++p) corr = fmaf(coef[p] * u[(int64_t)p * nc + n], v[p * vstride + (int64_t)t * kc + k], corr);
-    dwp[i] -= corr;
+    float* row = dwp + r * ld + k;
+    for (int c = 0; c < n_copies; ++c) row[(int64_t)c * kc] -= corr;
   }
+}
+
+// ---- row-strided power iteration with fixed-order sums (sg_snorm_sigma_ld) ------------------------------------
+// The matrix is M[t][n][k], k < kc, rows ld floats apart (ld > kc: one half of a tied [W | W] master).  No float
+// atomics: every sum is reduced in an order fixed by the launch geometry, so sigma, u and v have the same bits on
+// every run and every data-parallel rank that holds the same master.
+
+// every thread of a 256-thread block returns the block's sum (fixed order: warp trees, then warps 0..7)
+__device__ __forceinline__ float block_sum_256(float x, float* sh) {
+  x = warp_sum(x);
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = x;
+  __syncthreads();
+  float s = 0.f;
+  for (int i = 0; i < 8; ++i) s += sh[i];
+  __syncthreads();
+  return s;
+}
+
+// vraw[t][k] = sum_n M[t][n][k] * u[n] ;  part[block] = sum over the block's columns of vraw^2
+__global__ void __launch_bounds__(256)
+snorm_ld_wt_u_kernel(const float* __restrict__ m, int nc, int kc, int ld, const float* __restrict__ u,
+                     float* __restrict__ vraw, float* __restrict__ part) {
+  __shared__ float sh[8];
+  const int t = blockIdx.y;
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  float acc = 0.f;
+  if (k < kc) {
+    const float* p = m + (int64_t)t * nc * ld + k;
+    for (int n = 0; n < nc; ++n) acc = fmaf(p[(int64_t)n * ld], __ldg(u + n), acc);
+    vraw[(int64_t)t * kc + k] = acc;
+  }
+  const float s = block_sum_256(acc * acc, sh);
+  if (threadIdx.x == 0) part[(int64_t)blockIdx.y * gridDim.x + blockIdx.x] = s;
+}
+
+// uraw[n] = sum_{t,k} M[t][n][k] * vraw[t][k] / max(sqrt(*n2v), eps)   (block = one row n; n2v may be NULL)
+__global__ void __launch_bounds__(256)
+snorm_ld_w_v_kernel(const float* __restrict__ m, int T, int nc, int kc, int ld, const float* __restrict__ vraw,
+                    const float* __restrict__ n2v, float* __restrict__ uraw) {
+  __shared__ float sh[8];
+  const int n = blockIdx.x;
+  float acc = 0.f;
+  for (int t = 0; t < T; ++t) {
+    const float* p = m + ((int64_t)t * nc + n) * ld;
+    const float* v = vraw + (int64_t)t * kc;
+    for (int k = threadIdx.x; k < kc; k += 256) acc = fmaf(p[k], v[k], acc);
+  }
+  const float s = block_sum_256(acc, sh);
+  if (threadIdx.x == 0) uraw[n] = n2v ? s / fmaxf(sqrtf(*n2v), 1e-12f) : s;
+}
+
+// *out = sum_i a[i] * b[i]  (b NULL: sum_i a[i]); one 256-thread block
+__global__ void __launch_bounds__(256)
+snorm_ld_dot_kernel(const float* __restrict__ a, const float* __restrict__ b, int n, float* __restrict__ out) {
+  __shared__ float sh[8];
+  float acc = 0.f;
+  for (int i = threadIdx.x; i < n; i += 256) acc = b ? fmaf(a[i], b[i], acc) : acc + a[i];
+  const float s = block_sum_256(acc, sh);
+  if (threadIdx.x == 0) *out = s;
 }
 
 }  // namespace sg
@@ -154,7 +215,44 @@ extern "C" int sg_snorm_coef(const double* red, const float* bias, int C, const 
 extern "C" int sg_snorm_rank1(float* dwp, int n_taps, int nc, int kc, int n_pass, const float* u, const float* v,
                               const float* coef, void* stream) {
   SG_CHECK_ARG(dwp && u && v && coef && n_pass >= 1);
-  snorm_rank1_kernel<<<4 * NUM_SMS, 256, 0, ST>>>(dwp, n_taps, nc, kc, n_pass, u, v, coef);
+  snorm_rank1_kernel<<<4 * NUM_SMS, 256, 0, ST>>>(dwp, n_taps, nc, kc, kc, 1, n_pass, u, v, coef);
+  SG_CHECK_LAUNCH();
+  return SG_OK;
+}
+
+extern "C" int sg_snorm_rank1_ld(float* dwp, int n_taps, int nc, int kc, int ld, int n_copies, int n_pass,
+                                 const float* u, const float* v, const float* coef, void* stream) {
+  SG_CHECK_ARG(dwp && u && v && coef && n_pass >= 1 && n_copies >= 1 && ld >= n_copies * kc);
+  snorm_rank1_kernel<<<4 * NUM_SMS, 256, 0, ST>>>(dwp, n_taps, nc, kc, ld, n_copies, n_pass, u, v, coef);
+  SG_CHECK_LAUNCH();
+  return SG_OK;
+}
+
+// sg_snorm_sigma on the row-strided matrix M[t][n][k < kc] (rows ld floats apart), with fixed-order sums.
+// work: nc + n_taps * ceil(kc / 256) floats.
+extern "C" int sg_snorm_sigma_ld(const float* m, int n_taps, int nc, int kc, int ld, float* u, float* v, float* scal,
+                                 float* work, int training, void* stream) {
+  SG_CHECK_ARG(m && u && v && scal && work && n_taps >= 1 && nc > 0 && kc > 0 && ld >= kc);
+  const int nv = n_taps * kc;
+  if (training) {
+    dim3 g1((kc + 255) / 256, n_taps);
+    float* part = work + nc;
+    snorm_ld_wt_u_kernel<<<g1, 256, 0, ST>>>(m, nc, kc, ld, u, v, part);            // v <- W^T u (raw)
+    SG_CHECK_LAUNCH();
+    snorm_ld_dot_kernel<<<1, 256, 0, ST>>>(part, nullptr, (int)(g1.x * g1.y), scal + 0);
+    SG_CHECK_LAUNCH();
+    snorm_ld_w_v_kernel<<<nc, 256, 0, ST>>>(m, n_taps, nc, kc, ld, v, scal + 0, u);  // u <- W v / ||v|| (raw)
+    SG_CHECK_LAUNCH();
+    snorm_ld_dot_kernel<<<1, 256, 0, ST>>>(u, u, nc, scal + 1);
+    SG_CHECK_LAUNCH();
+    snorm_finish_kernel<<<((nv > nc ? nv : nc) + 255) / 256, 256, 0, ST>>>(u, nc, v, nv, scal, 1);
+  } else {
+    snorm_ld_w_v_kernel<<<nc, 256, 0, ST>>>(m, n_taps, nc, kc, ld, v, nullptr, work);
+    SG_CHECK_LAUNCH();
+    snorm_ld_dot_kernel<<<1, 256, 0, ST>>>(u, work, nc, scal + 1);
+    SG_CHECK_LAUNCH();
+    snorm_finish_kernel<<<1, 32, 0, ST>>>(u, nc, v, nv, scal, 0);
+  }
   SG_CHECK_LAUNCH();
   return SG_OK;
 }

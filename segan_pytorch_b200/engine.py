@@ -650,7 +650,9 @@ class _NetEngine:
                 self.index[name] = (off, p.numel(), tuple(p.shape))
                 off += (p.numel() + 3) // 4 * 4                  # 16-byte aligned views
         self.flat = torch.zeros(off, dtype=torch.float32, device=dev)
-        self.grad = torch.zeros(off, dtype=torch.float32, device=dev)
+        # the gradient bucket may carry a gradient-only tail past the parameters (_grad_tail): all-reduced with
+        # the gradients, never stepped by the optimiser (it steps flat.numel() elements)
+        self.grad = torch.zeros(off + self._grad_tail(), dtype=torch.float32, device=dev)
         self._mirror_ptr = {}
         for name, p in ps:
             p.grad = None
@@ -668,6 +670,9 @@ class _NetEngine:
         self._seen = self._versions()
         if hasattr(self, "sn"):
             self.sn = {}                     # spectral-norm state is rebuilt from the module's buffers
+
+    def _grad_tail(self):
+        return 0
 
     def _versions(self):
         return tuple(p._version for _, p in self.module.named_parameters())
@@ -835,10 +840,106 @@ class _NetEngine:
         self.pack_ev = {}
 
 
+# --------------------------------------------------------------------------------------------
+# spectral normalisation (norm_type='snorm', torch.nn.utils.spectral_norm) -- shared by both networks
+# --------------------------------------------------------------------------------------------
+def sn_v_layout(pl):
+    """(reference shape of weight_v as a weight with one output channel, c_in of that weight) of packed layer `pl`.
+    Conv1d (dim 0): v runs over (ci, k) -> [1][Cin][31]; ConvTranspose1d (dim 1): v runs over (ci, k) of
+    W[Cin][Cout][31] -> [Cin][1][31]; a tied master holds [W | W], whose v covers one half."""
+    vin = pl.c_in // 2 if pl.tied else pl.c_in
+    if pl.kind == 0:
+        return (1, vin, KW), vin
+    if pl.kind == 1:
+        return (vin, 1, KW), vin
+    return (1, -1), vin
+
+
+def sn_pack_v(pl, vref):
+    """weight_v (reference layout, flat) -> the packed slots the power iteration of `pl` runs on."""
+    shape, vin = sn_v_layout(pl)
+    return pack_reference(pl.kind, vref.reshape(shape), 1, vin, pl.t_len).reshape(-1).contiguous()
+
+
+def sn_unpack_v(pl, v):
+    return unpack_reference(pl.kind, v, 1, sn_v_layout(pl)[1], pl.t_len).reshape(-1)
+
+
+def sn_geometry(pl):
+    """(n_taps, nc, kc, ld) of the power iteration on the packed master of `pl` (include/segan_b200.h): kind 0 / 2
+    as packed (dim 0); kind 1 as [36][Cout][Cin] (dim 1: u per output channel); a tied master's first half."""
+    _, vin = sn_v_layout(pl)
+    if pl.kind == 1:
+        return 36, pl.c_out, vin, pl.kc
+    return pl.T, pl.nc, pl.kc, pl.kc
+
+
+class _SpectralNorm(object):
+    """Per-pass spectral-norm state of the normalised weights of a network (names ending in weight_orig): the
+    power-iteration vectors (u: the module's buffer itself; v: packed slots for the tap-GEMM layers, the module's
+    buffer for the small ones), per-pass copies of both, the per-pass [unused, unused, sigma, 1/sigma] scalars and
+    the per-pass sigma-term coefficients."""
+    SN_SLOTS = 5                    # up to 4 accumulating passes per optimiser step (WSEGAN) + 1 gradient-free pass
+
+    def _sn_coef(self, name):
+        """Storage of the per-pass sigma-term coefficients of packed layer `name` (SN_SLOTS floats)."""
+        return torch.zeros(self.SN_SLOTS, device=self.flat.device)
+
+    def _sn_state(self, name):
+        st = self.sn.get(name)
+        if st is not None:
+            return st
+        dev = self.flat.device
+        mod = dict(self.module.named_buffers())
+        base = name[:-len("weight_orig")]
+        u, vref = mod[base + "weight_u"], mod[base + "weight_v"]
+        pl = self.by_name.get(name)
+        if pl is not None:
+            T, nc, kc, ld = sn_geometry(pl)
+            v = sn_pack_v(pl, vref)
+        else:
+            # reference layout [height][rest]: dim 0, or dim 1 of a transposed conv with one output channel
+            nc = u.numel()
+            T, kc = 1, self.index[name][1] // nc
+            ld = kc
+            v = vref
+        P = self.SN_SLOTS
+        st = self.sn[name] = dict(T=T, nc=nc, kc=kc, ld=ld, u=u, v=v, vref=vref, pl=pl,
+                                  scal=torch.zeros(P, 4, device=dev), u_p=torch.zeros(P, nc, device=dev),
+                                  v_p=torch.zeros(P, T * kc, device=dev),
+                                  coef=self._sn_coef(name) if pl is not None else None,
+                                  work=torch.zeros(nc + T * ((kc + 255) // 256) + 4, device=dev),
+                                  seen=(u._version, vref._version))
+        return st
+
+    def _sn_master(self, name):
+        pl = self.by_name.get(name)
+        return self.mview(pl) if pl is not None else self.pview(name)
+
+    def sn_inv_sigma(self, name, slot=None):
+        """Device scalar 1 / sigma of `name` for pass slot `slot` (default: the current one)."""
+        return self._sn_state(name)["scal"][self._sn_slot if slot is None else slot][3:4]
+
+    def sync_to_reference(self):
+        super().sync_to_reference()
+        for name, st in self.sn.items():          # packed v -> the module's reference-layout buffer
+            pl = st["pl"]
+            if pl is not None:
+                st["vref"].copy_(sn_unpack_v(pl, st["v"]))
+                st["seen"] = (st["u"]._version, st["vref"]._version)
+
+    def _sn_fix_small(self, nm, scratch, slot):
+        """scratch gradient w.r.t. the normalised small tensor `nm` -> gradient w.r.t. weight_orig, into the bucket."""
+        stt = self._sn_state(nm)
+        _lib.call("sg_snorm_grad", _p(scratch), _p(self.pview(nm)), 1, stt["nc"], stt["kc"], _p(stt["u_p"][slot]),
+                  _p(stt["v_p"][slot]), _p(stt["scal"][slot]), _p(stt["work"][stt["nc"]:]), _stream())
+        self.gview(nm).add_(scratch)
+
+
 # ============================================================================================
 # Generator
 # ============================================================================================
-class GeneratorEngine(_NetEngine):
+class GeneratorEngine(_SpectralNorm, _NetEngine):
     def __init__(self, module):
         super().__init__(module)
         m = module
@@ -855,6 +956,29 @@ class GeneratorEngine(_NetEngine):
         self.conv_skip = self.has_skip and getattr(m, "skip_type", "alpha") == "conv"
         self.skip_kw = getattr(m, "skip_kwidth", 11)
         self.packed = {}
+        # norm_type='snorm' (modules.py:12-14): every encoder conv (dim 0) and decoder deconv (dim 1) is divided by its
+        # spectral norm, re-estimated by one power iteration per training forward; the parameters are then called
+        # weight_orig.  Skip convs and alphas are not normalised.
+        self.snorm = getattr(m, "norm_type", None) == "snorm"
+        self.wsfx = "_orig" if self.snorm else ""
+        self.sn = {}
+        self._sn_reset()
+
+    def _sn_reset(self):
+        # Pass slots: a forward that a backward will follow takes a slot that is neither outstanding (forward run,
+        # backward not yet) nor done (gradients in the bucket).  A step's G forward runs BEFORE Gopt.zero_grad()
+        # (SEGAN / WSEGAN), so zero_grad() drops only the done slots.  The done slots' sigma terms are applied in
+        # finish_grads().
+        self._sn_live = {}          # slot -> ticket of the outstanding forward that holds it
+        self._sn_done = []          # slots whose gradients are in the bucket
+        self._sn_ticket = 0
+        self._sn_slot = self.SN_SLOTS - 1
+        self._sn_eval_ok = False    # the operands hold the eval-mode sigma of the current masters and vectors
+        self._ops_slot = None       # the pass slot whose 1 / sigma the current 16-bit operands carry
+
+    def wname(self, block, l):
+        """Name of the weight of encoder ('enc') or decoder ('dec') block l (weight_orig with snorm)."""
+        return ("enc_blocks.%d.conv.weight%s" if block == "enc" else "dec_blocks.%d.deconv.weight%s") % (l, self.wsfx)
 
     # -- weights ----------------------------------------------------------------------------
     def packed_layers(self):
@@ -864,14 +988,94 @@ class GeneratorEngine(_NetEngine):
         fm, nl = self.fmaps, self.nl
         ls = []
         for l in range(nl - 1):
-            ls.append(PackedLayer("dec_blocks.%d.deconv.weight" % l, 1, self.dec_cout(l), self.dec_cin(l), 0,
+            ls.append(PackedLayer(self.wname("dec", l), 1, self.dec_cout(l), self.dec_cin(l), 0,
                                   "Wt%d" % l, "Wtd%d" % l,
                                   alpha_name=(("alpha_%d.skip_k" % (nl - 1 - l))
                                               if l > 0 and self.has_skip and not self.conv_skip else None),
                                   tied=(self.sum_merge and l > 0)))
-        ls += [PackedLayer("enc_blocks.%d.conv.weight" % l, 0, fm[l], fm[l - 1], 0, "Wf%d" % l, "Wdg%d" % l)
+        ls += [PackedLayer(self.wname("enc", l), 0, fm[l], fm[l - 1], 0, "Wf%d" % l, "Wdg%d" % l)
                for l in range(nl - 1, 0, -1)]
         return ls
+
+    # -- spectral norm (state: _SpectralNorm) ------------------------------------------------------
+    def _sn_names(self):
+        return [self.wname("enc", l) for l in range(self.nl)] + [self.wname("dec", l) for l in range(self.nl)]
+
+    def _grad_tail(self):
+        """snorm: the per-pass sigma-term coefficients of the packed layers ride at the end of the gradient bucket, so
+        that the data-parallel all-reduce sums them with the gradients: the sigma terms applied after it
+        (finish_grads) then use the coefficients of the whole batch."""
+        return len(self.layers) * self.SN_SLOTS if self.snorm else 0
+
+    def _sn_coef(self, name):
+        i = self.layers.index(self.by_name[name])
+        o = self.flat.numel() + i * self.SN_SLOTS
+        return self.grad[o:o + self.SN_SLOTS]
+
+    def _build(self, ps, dev):
+        super()._build(ps, dev)
+        self._sn_reset()
+
+    def _sn_iterate(self, training, slot):
+        """sigma of every normalised weight for the coming pass (one power iteration when training) into pass slot
+        `slot`, with copies of the vectors for that pass's backward.  sg_snorm_sigma_ld sums in a fixed order: ranks
+        holding the same masters and vectors compute the same bits, so u, v and sigma never drift apart."""
+        st_ = _stream()
+        for name in self._sn_names():
+            st = self._sn_state(name)
+            _lib.call("sg_snorm_sigma_ld", _p(self._sn_master(name)), st["T"], st["nc"], st["kc"], st["ld"], _p(st["u"]),
+                      _p(st["v"]), _p(st["scal"][slot]), _p(st["work"]), 1 if training else 0, st_)
+            st["u_p"][slot].copy_(st["u"])
+            st["v_p"][slot].copy_(st["v"].reshape(-1))
+        self._sn_slot = slot
+
+    def _sn_take_slot(self):
+        """Pass slot of a forward that a backward will follow (see _sn_reset).  With every slot taken, the oldest
+        outstanding forward's slot is reused: its backward then raises."""
+        busy = set(self._sn_live) | set(self._sn_done)
+        free = [s for s in range(self.SN_SLOTS - 1) if s not in busy]
+        if free:
+            slot = free[0]
+        elif self._sn_live:
+            slot = min(self._sn_live, key=self._sn_live.get)
+        else:
+            raise RuntimeError("more than %d accumulating Generator passes per optimiser step" % (self.SN_SLOTS - 1))
+        self._sn_ticket += 1
+        self._sn_live[slot] = self._sn_ticket
+        return slot, self._sn_ticket
+
+    def _sn_notice_buffers(self):
+        """weight_u / weight_v written through torch (load_state_dict, copy_): the packed v is re-imported in place
+        and the operands are re-emitted with the new sigma."""
+        for st in self.sn.values():
+            seen = (st["u"]._version, st["vref"]._version)
+            if seen != st["seen"]:
+                if st["pl"] is not None:
+                    st["v"].copy_(sn_pack_v(st["pl"], st["vref"]))
+                st["seen"] = seen
+                self._ops_stale, self._sn_eval_ok = True, False
+
+    def notice_external_writes(self):
+        super().notice_external_writes()
+        if self.snorm:
+            self._sn_notice_buffers()
+
+    def master_updated(self):
+        super().master_updated()
+        self._sn_eval_ok = False
+
+    def zero_grad(self):
+        super().zero_grad()
+        self._sn_done = []
+
+    def grads_consumed(self, cleared):
+        super().grads_consumed(cleared)
+        if cleared:
+            self._sn_done = []
+            if self.snorm:
+                # the optimiser clears the parameters' gradients only: clear the coefficient tail too, so that no stale
+                # value is all-reduced (and multiplied by the world size) step after step
+                self.grad[self.flat.numel():].zero_()
 
     def grad_chunks(self):
         """[(offset, numel)]: decoder weights (complete after dec0's weight gradient) | enc_{nl-1} | the rest."""
@@ -881,10 +1085,16 @@ class GeneratorEngine(_NetEngine):
 
     def pack(self):
         dev = self.flat.device
-        # last decoder layer (Cout = 1): fp32 [cin][31] with alpha folded (tiny: torch ops)
+        # last decoder layer (Cout = 1): fp32 [cin][31] with alpha folded (tiny: torch ops); snorm: every operand below
+        # and the waveform-end conv's are made of W / sigma
         l = self.nl - 1
-        w = self.pview("dec_blocks.%d.deconv.weight" % l)[:, 0, :]
-        if self.sum_merge:                       # tied halves: W (hi + alpha skip) = [W | alpha W] cat(hi, skip)
+        w = self.pview(self.wname("dec", l))[:, 0, :]
+        w0 = self.pview(self.wname("enc", 0))
+        if self.snorm:
+            self._ops_slot = self._sn_slot
+            w = w * self.sn_inv_sigma(self.wname("dec", l))
+            w0 = w0 * self.sn_inv_sigma(self.wname("enc", 0))
+        if self.sum_merge:                      # tied halves: W (hi + alpha skip) = [W | alpha W] cat(hi, skip)
             w = torch.cat((w, w), 0)
         self.packed["w_last_dup"] = w.reshape(w.shape[0], 1, KW).contiguous()
         weff = w.clone()
@@ -893,7 +1103,7 @@ class GeneratorEngine(_NetEngine):
             weff[half:] = weff[half:] * self.alpha_for_dec(l).view(-1, 1)
         self.packed["w_last_eff"] = weff.contiguous()
         # tensor-core route of the waveform-end layers: single-tap operands (tiny tensors, torch ops)
-        wcol = wave_col_weights(self.pview("enc_blocks.0.conv.weight"), dev)
+        wcol = wave_col_weights(w0, dev)
         self.packed["Wcol0"] = wcol.half().contiguous()
         kidx = dec_last_tap_index(dev)
         w2 = weff.t()[kidx.clamp(min=0)] * (kidx >= 0).float().unsqueeze(1)       # [64][cin]
@@ -914,11 +1124,23 @@ class GeneratorEngine(_NetEngine):
                 self.packed["Wsk%d" % l], self.packed["Wskd%d" % l] = wf, wd
                 self._mark_packed("Wsk%d" % l)
         for pl in self.layers:
-            self.emit(pl, self.pview(pl.alpha_name).reshape(-1) if pl.alpha_name else None)
+            self.emit(pl, self.pview(pl.alpha_name).reshape(-1) if pl.alpha_name else None,
+                      scale=self.sn_inv_sigma(pl.name) if self.snorm else None)
 
     def finish_grads(self):
+        """Per packed layer, in this order: the alpha fix (dWeff -> dW and dalpha), the sum of the tied halves, and with
+        snorm the sigma terms of the step's passes.  Each pass's weight-gradient GEMM scaled by 1/sigma_p, so the
+        alpha fix against the master W gives sum_p <dWeff_p, W / sigma_p> = dalpha, and afterwards the bucket holds
+        sum_p (dL/dW~_p) / sigma_p, from which sg_snorm_rank1_ld subtracts sum_p coef_p u_p v_p^T (on both tied
+        copies).  The sigma term must come after the alpha fix: the fix multiplies the skip columns by alpha."""
         if self._alpha_fixed:
             return
+        runs = []
+        for s in sorted(self._sn_done) if self.snorm else ():
+            if runs and runs[-1][0] + runs[-1][1] == s:
+                runs[-1][1] += 1
+            else:
+                runs.append([s, 1])
         for pl in self.layers:
             if pl.alpha_name is not None:
                 trainable = self._param(pl.alpha_name).requires_grad
@@ -930,6 +1152,12 @@ class GeneratorEngine(_NetEngine):
                 tot = g2[:, :, 0] + g2[:, :, 1]
                 g2[:, :, 0] = tot
                 g2[:, :, 1] = tot
+            if runs:
+                st = self._sn_state(pl.name)
+                for s0, n in runs:
+                    _lib.call("sg_snorm_rank1_ld", _p(self.mgrad(pl)), st["T"], st["nc"], st["kc"], st["ld"],
+                              2 if pl.tied else 1, n, _p(st["u_p"][s0]), _p(st["v_p"][s0]), _p(st["coef"][s0:]),
+                              _stream())
         self._alpha_fixed = True
 
     def dec_cin(self, l):
@@ -956,17 +1184,34 @@ class GeneratorEngine(_NetEngine):
         return self.pview("alpha_%d.skip_k" % (self.nl - 1 - l)).reshape(-1)
 
     # -- forward ----------------------------------------------------------------------------
-    def forward(self, x, z, want_ctx=True, fresh=False, twins=None):
+    def forward(self, x, z, want_ctx=True, fresh=False, twins=None, training=True):
         """x: (B,1,L) fp32 cuda, z: (B, C4, L/1024) fp32 cuda.  Returns y (B,1,L) fp32.
         twins (default = want_ctx): also write the bf16 copies of the activations that only the weight-gradient
         tap-GEMMs read; inference passes False (one store per activation instead of two or three).
         fresh=True gives the saved activations their own storage (generic autograd use, where several
-        forwards may precede a backward); the fused train step reuses one persistent workspace."""
+        forwards may precede a backward); the fused train step reuses one persistent workspace.
+        training (snorm only, the module's mode): one power iteration that updates weight_u / weight_v; eval mode
+        uses the stored vectors and leaves them unchanged."""
         _require_cuda(x, z)
         twins = want_ctx if twins is None else (twins and want_ctx)
         bwd = twins                               # a backward pass will read this forward's saved tensors
         alias = twins and not grad_twins()        # fp16 gradients: the weight-gradient GEMMs read the forward tensors
         twins = twins and grad_twins()
+        sn_slot = None
+        if self.snorm:
+            if not wave_on_tensor_cores():
+                raise NotImplementedError("norm_type='snorm' needs the tensor-core waveform route (SEGAN_B200_WAVE=tc)")
+            self.bind()
+            self.notice_external_writes()
+            if bwd:
+                sn_slot = self._sn_take_slot()
+                self._sn_iterate(training, sn_slot[0])
+                self._ops_stale, self._sn_eval_ok = True, False
+            elif training or not self._sn_eval_ok or self._ops_stale:
+                # gradient-free pass: slot SN_SLOTS - 1; an eval-mode sigma stays valid until the masters or the
+                # vectors change
+                self._sn_iterate(training, self.SN_SLOTS - 1)
+                self._ops_stale, self._sn_eval_ok = True, not training
         self.ensure_packed()
         self.wait_packed("small")
         B, _, L = x.shape
@@ -1097,7 +1342,7 @@ class GeneratorEngine(_NetEngine):
                       _p(self.packed["w_last_eff"]), _p(blast), _p(y), st)
         self.packs_consumed()
         ctx = dict(x=x, B=B, L=L, Lq=Lq, a=a, hp=hp, z16=z16, ad=ad, dd=dd, y=y, hpb=hpb, ab=ab, ddb=ddb,
-                   z16b=z16b, colb=colb, skb=skb if self.conv_skip else ab) if want_ctx else None
+                   z16b=z16b, colb=colb, skb=skb if self.conv_skip else ab, sn_slot=sn_slot) if want_ctx else None
         return y, ctx
 
     def _skip_conv_fwd(self, l, a_l, B, lq, buf, twins, alias):
@@ -1156,9 +1401,43 @@ class GeneratorEngine(_NetEngine):
         a, hp, ad, dd = ctx["a"], ctx["hp"], ctx["ad"], ctx["dd"]
         dev = gy.device
         gy = gy.contiguous().float()
+        slot, sn_small = None, {}
+        if self.snorm:
+            slot, ticket = ctx["sn_slot"]
+            if self._sn_live.get(slot) != ticket:
+                raise RuntimeError("this Generator forward's spectral-norm state was reused by %d later forward passes "
+                                   "that kept their graphs: run at most %d forward passes ahead of their backward "
+                                   "passes" % (self.SN_SLOTS - 1, self.SN_SLOTS - 1))
+        if self.snorm and self._ops_slot != slot:
+            # another forward (a second outstanding pass, or a gradient-free training pass) re-emitted the operands with
+            # its own sigma since this pass's forward: the data-gradient GEMMs and the last block's fold read W / sigma
+            # of THIS pass, so the operands are emitted again for its slot, in line on this stream
+            self.packs_consumed()
+            self._sn_slot = slot
+            self.pack()
+            self._sn_eval_ok = False
         if not accumulate:
             self.zero_grad()
         self._grad_dirty = True
+        if self.snorm:
+            del self._sn_live[slot]
+            self._sn_done.append(slot)
+            # the waveform ends are small tensors: this pass's gradient w.r.t. W / sigma goes to a scratch buffer and
+            # sg_snorm_grad turns it into the weight_orig gradient (_sn_fix_small)
+            for nm in (self.wname("enc", 0), self.wname("dec", nl - 1)):
+                sn_small[nm] = buf.get("g.sng." + nm, self.index[nm][2], F32, dev, zero=True)
+
+        def wgrad_dst(nm):
+            """Where this pass's gradient of the small weight `nm` is accumulated."""
+            return sn_small[nm] if nm in sn_small else self.gview(nm)
+
+        def sn_coef(red, bias, c, pl_name):
+            """snorm: sigma-term coefficient <dL/dW~, W~> / sigma of this pass from the layer's output statistics."""
+            if self.snorm:
+                stt = self._sn_state(pl_name)
+                _lib.call("sg_snorm_coef", _p(red), _p(bias), c, _p(stt["scal"][slot]), _p(stt["coef"][slot:slot + 1]),
+                          st)
+        osc = (lambda nm: self.sn_inv_sigma(nm, slot)) if self.snorm else (lambda nm: None)
         side = side_stream(dev, 0)       # weight-gradient tap-GEMM of every layer (writes the packed gradient bucket)
         red_dec = stat_arena(buf, "g.red_dec", [(SL, 3, self.dec_cout(l)) for l in range(nl - 1)], dev)
         red_enc = stat_arena(buf, "g.red_enc", [(SL, 3, fm[l]) for l in range(nl)], dev)
@@ -1196,22 +1475,27 @@ class GeneratorEngine(_NetEngine):
                     run_w(colg, lin // 2, GS, ctx["ddb"][l - 1], None, lin // 2, 0, GS, 2 * cin, 128,
                           tap_ranges("full", 0, 2 * cin, 128), dwq, B, d_lo=0, d_hi=0, dw_tap0=4, ksplit=74,
                           a0_c=2 * cin, backend=self.backend)
-                    _lib.call("sg_last_deconv_wgrad_fold_1src", _p(dwq), cin,
-                              _p(self.gview("dec_blocks.%d.deconv.weight" % l)), _stream())
+                    _lib.call("sg_last_deconv_wgrad_fold_1src", _p(dwq), cin, _p(wgrad_dst(self.wname("dec", l))),
+                              _stream())
+                    if sn_small:
+                        self._sn_fix_small(self.wname("dec", l), sn_small[self.wname("dec", l)], slot)
             else:
                 a_train = not self.conv_skip and self._param("alpha_0.skip_k").requires_grad
                 with on_side(side):
                     run_w(colg, lin // 2, GS, ctx["ddb"][l - 1], ctx["skb"][0], lin // 2, 0, GS, 2 * cin, 128,
                           tap_ranges("full", 0, 2 * cin, 128), dwq, B, d_lo=0, d_hi=0, dw_tap0=4, ksplit=74,
                           a0_c=cin, a1_c=cin, backend=self.backend)
-                    gw_dst = self.gview("dec_blocks.%d.deconv.weight" % l)
+                    gw_dst = wgrad_dst(self.wname("dec", l))
                     if self.sum_merge:
                         gw_dst = buf.get("g.gw_last2", (cin, 1, KW), F32, dev, zero=True)
+                    # snorm: w_last_dup is W / sigma, so the fold's dalpha is <dWeff, W~> as the reference's
                     _lib.call("sg_last_deconv_wgrad_fold", _p(dwq), half, _p(self.packed["w_last_dup"]),
                               _p(self.alpha_for_dec(l)), _p(gw_dst),
                               _p(self.gview("alpha_0.skip_k").view(-1)) if a_train else None, _stream())
                     if self.sum_merge:
-                        self.gview("dec_blocks.%d.deconv.weight" % l).add_(gw_dst[:half] + gw_dst[half:])
+                        wgrad_dst(self.wname("dec", l)).add_(gw_dst[:half] + gw_dst[half:])
+                    if sn_small:
+                        self._sn_fix_small(self.wname("dec", l), sn_small[self.wname("dec", l)], slot)
         else:
             if not self.has_skip:
                 raise NotImplementedError("a Generator without skips (skip=False) needs the tensor-core waveform "
@@ -1242,18 +1526,19 @@ class GeneratorEngine(_NetEngine):
                       None, None, _p(self.pview("dec_blocks.%d.act.weight" % l)), ACT_PRELU, _p(red), _p(g_ad), st)
             _lib.call("sg_stat_grads", _p(red), cout, 3, _p(self.gview("dec_blocks.%d.act.weight" % l)),
                       _p(self.gview("dec_blocks.%d.deconv.bias" % l)), None, st)
+            sn_coef(red, self.pview("dec_blocks.%d.deconv.bias" % l), cout, self.wname("dec", l))
             if l == 0:
                 s0, s1 = (ctx["z16b"], ctx["hpb"][nl - 1]) if self.zc else (ctx["hpb"][nl - 1], None)
             else:
                 s0, s1 = ctx["ddb"][l - 1], (ctx["skb"][nl - 1 - l] if self.has_skip else None)
             c0, c1 = s0.shape[-1], (0 if s1 is None else s1.shape[-1])
             taps = tap_ranges("deconv_fwd", cout, cin, 4 * cout)
-            dwp = self.mgrad(self.by_name["dec_blocks.%d.deconv.weight" % l])     # packed gradient slot (dWeff)
+            dwp = self.mgrad(self.by_name[self.wname("dec", l)])     # packed gradient slot (dWeff; snorm: / sigma)
             with on_side(side):
                 n_tiles = 9 * (4 * cout // 128) * max(1, cin // 256)
                 run_w(g_ad, lin, GS, s0, s1, lin, 0, GS, cin, 4 * cout, taps, dwp, B,
                       ksplit=wgrad_ksplit(B * lin, n_tiles, taps, cin, 4 * cout), a0_c=c0, a1_c=c1,
-                      backend=self.backend)
+                      backend=self.backend, out_scale=osc(self.wname("dec", l)))
                 if l == 0 and reducer is not None:
                     reducer.ready(0, launch=True)              # every decoder weight gradient has been enqueued
             # data gradient w.r.t. cat(s0, s1); block 0 only needs the code's columns [zc, zc + C) (z gets no
@@ -1301,18 +1586,23 @@ class GeneratorEngine(_NetEngine):
                         run_w(g_a, Lq[0] // 2, GS, ctx["colb"], None, Lq[0] // 2, 0, GS, 128, 128,
                               tap_ranges("full", 0, 128, 128), dwq, B, d_lo=0, d_hi=0, dw_tap0=4, ksplit=148,
                               backend=self.backend)
-                        _lib.call("sg_wave_wgrad_fold", _p(dwq), 1, _p(self.gview("enc_blocks.0.conv.weight")), _stream())
+                        _lib.call("sg_wave_wgrad_fold", _p(dwq), 1, _p(wgrad_dst(self.wname("enc", 0))), _stream())
                     else:
                         _lib.call("sg_wave_conv_wgrad", _p(ctx["x"]), None, 1, B, L, 0, _p(g_a), cout,
                                   _p(self.gview("enc_blocks.0.conv.weight")), None, _stream())
+                    if sn_small:
+                        self._sn_fix_small(self.wname("enc", 0), sn_small[self.wname("enc", 0)], slot)
                 break
+            sn_coef(red, self.pview("enc_blocks.%d.conv.bias" % l) if self.enc_bias else None, cout,
+                    self.wname("enc", l))
             cin = fm[l - 1]
             taps = tap_ranges("conv_fwd", cin, 4 * cin, cout)
-            dwp_l = self.mgrad(self.by_name["enc_blocks.%d.conv.weight" % l])
+            dwp_l = self.mgrad(self.by_name[self.wname("enc", l)])
             with on_side(side):
                 n_tiles = 9 * (cout // 128) * max(1, 4 * cin // 256)
                 run_w(g_a, Lq[l], GS, ctx["hpb"][l - 1], None, Lq[l], 4, GS, 4 * cin, cout, taps, dwp_l, B,
-                      ksplit=wgrad_ksplit(B * Lq[l], n_tiles, taps, 4 * cin, cout), backend=self.backend)
+                      ksplit=wgrad_ksplit(B * Lq[l], n_tiles, taps, 4 * cin, cout), backend=self.backend,
+                      out_scale=osc(self.wname("enc", l)))
                 if l == nl - 1 and reducer is not None:
                     reducer.ready(1, launch=True)
             g_hp = buf.get("g.ghp%d" % (l - 1), (B, Lq[l] + 8, 4 * cin), GT, dev)
@@ -1356,7 +1646,7 @@ class GeneratorEngine(_NetEngine):
 # ============================================================================================
 # Discriminator
 # ============================================================================================
-class DiscriminatorEngine(_NetEngine):
+class DiscriminatorEngine(_SpectralNorm, _NetEngine):
     def __init__(self, module):
         super().__init__(module)
         self.fmaps = list(module.fmaps)
@@ -1395,8 +1685,7 @@ class DiscriminatorEngine(_NetEngine):
                for l in range(self.nl - 1, 0, -1)]
         return ls
 
-    # -- spectral norm ----------------------------------------------------------------------------
-    SN_SLOTS = 5                    # up to 4 accumulating passes per optimiser step (WSEGAN) + 1 gradient-free pass
+    # -- spectral norm (state: _SpectralNorm) ------------------------------------------------------
     # the head's spectrally normalised tensors (discriminator.py:118-121,125-137)
     HEAD_SN = {"none": ("fc.0.weight_orig", "fc.2.weight_orig", "fc.3.weight_orig"),
                "conv": ("pool_conv.weight_orig", "fc.weight_orig"), "gmax": ("fc.weight_orig",),
@@ -1404,38 +1693,6 @@ class DiscriminatorEngine(_NetEngine):
 
     def _sn_names(self):
         return ["enc_blocks.%d.conv.weight_orig" % l for l in range(self.nl)] + list(self.HEAD_SN[self.pool_type])
-
-    def _sn_state(self, name):
-        """Spectral-norm state of one weight: the power-iteration vectors (u: the module's buffer itself; v: packed
-        slots for the tap-GEMM layers, the module's buffer for the small ones), per-pass copies of both, the
-        per-pass [unused, unused, sigma, 1/sigma] scalars and the per-pass sigma-term coefficients."""
-        st = self.sn.get(name)
-        if st is not None:
-            return st
-        dev = self.flat.device
-        mod = dict(self.module.named_buffers())
-        base = name[:-len("weight_orig")]
-        u, vref = mod[base + "weight_u"], mod[base + "weight_v"]
-        pl = self.by_name.get(name)
-        if pl is not None:
-            T, nc, kc = pl.T, pl.nc, pl.kc
-            # v lives in packed slots: the same transform that packs a weight with one output channel
-            v = pack_reference(pl.kind, vref.reshape(1, -1) if pl.kind == 2 else vref.reshape(1, pl.c_in, KW), 1,
-                               pl.c_in, pl.t_len).reshape(-1).contiguous()
-        else:
-            shape = self.index[name][2]
-            T, nc, kc = 1, shape[0], int(torch.Size(shape[1:]).numel()) if len(shape) > 1 else 1
-            v = vref
-        P = self.SN_SLOTS
-        st = self.sn[name] = dict(T=T, nc=nc, kc=kc, u=u, v=v, vref=vref, pl=pl,
-                                  scal=torch.zeros(P, 4, device=dev), u_p=torch.zeros(P, nc, device=dev),
-                                  v_p=torch.zeros(P, T * kc, device=dev), coef=torch.zeros(P, device=dev),
-                                  work=torch.zeros(nc + 4, device=dev))
-        return st
-
-    def _sn_master(self, name):
-        pl = self.by_name.get(name)
-        return self.mview(pl) if pl is not None else self.pview(name)
 
     def _sn_iterate(self, training, slot):
         """sigma of every normalised weight for the coming pass (one power iteration when training), kept in pass
@@ -1448,17 +1705,6 @@ class DiscriminatorEngine(_NetEngine):
             st["u_p"][slot].copy_(st["u"])
             st["v_p"][slot].copy_(st["v"].reshape(-1))
         self._sn_slot = slot
-
-    def sn_inv_sigma(self, name, slot=None):
-        """Device scalar 1 / sigma of `name` for pass slot `slot` (default: the current one)."""
-        return self._sn_state(name)["scal"][self._sn_slot if slot is None else slot][3:4]
-
-    def sync_to_reference(self):
-        super().sync_to_reference()
-        for name, st in self.sn.items():          # packed v -> the module's reference-layout buffer
-            pl = st["pl"]
-            if pl is not None:
-                st["vref"].copy_(unpack_reference(pl.kind, st["v"], 1, pl.c_in, pl.t_len).reshape(-1))
 
     def zero_grad(self):
         super().zero_grad()
@@ -1725,13 +1971,6 @@ class DiscriminatorEngine(_NetEngine):
         if param_grads and self.snorm:
             for nm in self.HEAD_SN[self.pool_type]:
                 self._sn_fix_small(nm, g[nm[:-len("_orig")]], slot)
-
-    def _sn_fix_small(self, nm, scratch, slot):
-        """scratch gradient w.r.t. the normalised small tensor `nm` -> gradient w.r.t. weight_orig, into the bucket."""
-        stt = self._sn_state(nm)
-        _lib.call("sg_snorm_grad", _p(scratch), _p(self.pview(nm)), 1, stt["nc"], stt["kc"], _p(stt["u_p"][slot]),
-                  _p(stt["v_p"][slot]), _p(stt["scal"][slot]), _p(stt["work"][stt["nc"]:]), _stream())
-        self.gview(nm).add_(scratch)
 
     def backward(self, ctx, target, weight=1.0, param_grads=True, input_grad=None, loss_out=None, g_logit=None,
                  input_grad1=None, reducer=None, reduce_now=True):

@@ -2,7 +2,8 @@
 
 Same constructor signature, same `forward(x, z=None, ret_hid=False)` contract, same state-dict
 keys; the arithmetic runs in libsegan_b200.so (segan_pytorch_b200.engine.GeneratorEngine).  Served: alpha / constant /
-conv skips with concat or sum merge, skip=False, no_z=True and any z_dim that is a positive multiple of 64."""
+conv skips with concat or sum merge, skip=False, no_z=True, any z_dim that is a positive multiple of 64, and
+norm_type None or 'snorm' (spectrally normalised encoder convs and decoder deconvs)."""
 import torch
 import torch.nn as nn
 
@@ -56,8 +57,8 @@ class _GeneratorFn(torch.autograd.Function):
     """Whole-network autograd node: forward / backward are the fused kernel pipelines."""
 
     @staticmethod
-    def forward(ctx, eng, x, z, *params):
-        y, ectx = eng.forward(x, z, fresh=True)
+    def forward(ctx, eng, x, z, training, *params):
+        y, ectx = eng.forward(x, z, fresh=True, training=training)
         ctx.eng, ctx.ectx = eng, ectx
         eng._last_ctx = ectx
         ctx.names = [n for n, p in eng.module.named_parameters()]
@@ -71,7 +72,7 @@ class _GeneratorFn(torch.autograd.Function):
         grads = []
         for n, p in eng.module.named_parameters():
             grads.append(eng.grad_of(n) if p.requires_grad else None)      # reference layout, true units
-        return (None, None, None) + tuple(grads)
+        return (None, None, None, None) + tuple(grads)
 
 
 class Generator(Model):
@@ -142,13 +143,18 @@ class Generator(Model):
                                                        and (skip_type in ('alpha', 'constant')
                                                             or (skip_type == 'conv'
                                                                 and _engine.skipconv_served(skip_kwidth)))))
-                        and norm_type is None
+                        and norm_type in (None, 'snorm')
                         and all(k == 31 for k in kwidth) and all(k == 31 for k in dec_kwidth)
                         and all(p == 4 for p in poolings) and all(p == 4 for p in dec_poolings)
                         and list(dec_fmaps) == fmaps[::-1][1:] + [1]
                         and all(f % 64 == 0 for f in fmaps) and fmaps[0] == 64)
+        self.norm_type = norm_type
         self._unserved = None if self._served else ("this Generator configuration is outside the built hot path "
-                                                     "(SEGAN+ layout: k=31, stride 4, no norm, fmaps 64..)")
+                                                     "(SEGAN+ layout: k=31, stride 4, norm_type None or 'snorm', "
+                                                     "fmaps 64..)")
+        if norm_type == 'bnorm':
+            self._unserved = ("norm_type='bnorm' is not served for the Generator: the Generator's kernels have no "
+                              "BatchNorm between a convolution and its PReLU (norm_type None and 'snorm' are served)")
         if self.z_dim is None and not no_z:
             self.z_dim = fmaps[-1]
         if self._served and not no_z and not (isinstance(self.z_dim, int) and self.z_dim > 0 and self.z_dim % 64 == 0):
@@ -200,11 +206,12 @@ class Generator(Model):
         eng.bind()
         if torch.is_grad_enabled() and any(p.requires_grad for p in super().parameters()):
             params = [p for _, p in self.named_parameters()]
-            y = _GeneratorFn.apply(eng, x, z, *params)
+            y = _GeneratorFn.apply(eng, x, z, self.training, *params)
             ectx = eng._last_ctx          # hidden activations are exposed detached (inspection only)
             eng._last_ctx = None
         else:
-            y, ectx = eng.forward(x, z, twins=False)      # inference: no bf16 twins for weight gradients
+            # inference: no bf16 twins for weight gradients
+            y, ectx = eng.forward(x, z, twins=False, training=self.training)
         if ret_hid:
             # ret_hid may be an iterable of keys (additive): only those activations are converted to NCL
             only = None if ret_hid is True else set(ret_hid)

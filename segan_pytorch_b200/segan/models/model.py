@@ -700,7 +700,7 @@ class SEGAN(Model):
                 fwd_real_done = torch.cuda.Event()
                 fwd_real_done.record()
             de.backward(c, 1.0, 1.0, param_grads=True, loss_out=lptr(0), reducer=reducer, reduce_now=False)
-        Genh, gctx = ge.forward(noisy, z)
+        Genh, gctx = ge.forward(noisy, z, training=self.G.training)
         if fwd_real_done is not None:
             # BatchNorm running statistics are updated real pass first, fake pass second (model.py:297,303)
             torch.cuda.current_stream().wait_event(fwd_real_done)
@@ -746,7 +746,7 @@ class SEGAN(Model):
         key = (B, L, float(l1_weight), Gopt.param_groups[0]['lr'], Dopt.param_groups[0]['lr'], world,
                ge.flat.data_ptr() if ge.flat is not None else 0, de.flat.data_ptr() if de.flat is not None else 0,
                _engine.OVERLAP, self.z_device, bool(sample_z), ge.backend, de.backend, _engine.GS,
-               _engine.LOSS_SCALE)
+               _engine.LOSS_SCALE, ge.snorm and self.G.training)
         cache = self.__dict__.setdefault('_step_graphs', {})
         st = cache.get(key)
         if st is None:
@@ -1095,7 +1095,7 @@ class WSEGAN(SEGAN):
         # the G forward (model.py:583) does not depend on the D(real) pass before it: side stream 1
         gside = _engine.side_stream(dev, 1)
         with _engine.on_side(gside):
-            Genh, gctx = ge.forward(noisy, z)
+            Genh, gctx = ge.forward(noisy, z, training=self.G.training)
         Dopt.zero_grad()
         rd, rg = self._reducers()
         n_d = 2 + int(bool(self.misalign_pair)) + int(bool(self.interf_pair))      # the last D pass launches the chunks
@@ -1165,7 +1165,8 @@ class WSEGAN(SEGAN):
         key = ('w', B, L, Gopt.param_groups[0]['lr'], Dopt.param_groups[0]['lr'], world,
                ge.flat.data_ptr() if ge.flat is not None else 0, de.flat.data_ptr() if de.flat is not None else 0,
                _engine.OVERLAP, self.z_device, bool(sample_z), ge.backend, de.backend, _engine.GS, _engine.LOSS_SCALE,
-               bool(self.misalign_pair), bool(self.interf_pair), float(self.pow_weight), n_pass)
+               bool(self.misalign_pair), bool(self.interf_pair), float(self.pow_weight), n_pass,
+               ge.snorm and self.G.training)
         cache = self.__dict__.setdefault('_step_graphs', {})
         st = cache.get(key)
         if st is None:
