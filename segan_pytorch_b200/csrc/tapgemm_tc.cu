@@ -3,9 +3,10 @@
 // Both kernels are persistent (at most one CTA per SM, static round-robin tile schedule) and warp
 // specialised by warpgroup -- warpgroup 0: TMA producer (one thread issues, the others give their
 // registers back with setmaxnreg), warpgroups 1 and 2: consumers, each owning 64 of the tile's 128 M rows
-// with its fp32 accumulator in registers (wgmma m64nNk16, N = the tile's width) and storing its own rows
-// in the epilogue.  A 4-stage shared-memory ring (full / empty mbarriers) keeps the producer ahead of
-// the consumers, so the loads of tile i+1 overlap the epilogue of tile i.
+// with its fp32 accumulator in registers (wgmma m64nNk16, N = the tile's width).  A 4-stage shared-memory
+// ring (full / empty mbarriers) keeps the producer ahead of the consumers, so the loads of tile i+1 overlap
+// the epilogue of tile i.  Form F stages whole 16-bit output tiles in shared memory and writes them with TMA
+// stores that drain during the next tile's MMAs (f_epilogue_tma); the other epilogues store from the fragment.
 //
 // Every operand tile is a TMA box of 64 channels (128 B) x rows, 128B-swizzled, so the same
 // shared-memory bytes serve as
@@ -80,6 +81,25 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, u
 }
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
+}
+// TMA tensor store shared -> global (bulk async-group of the issuing thread); the box is clipped at the map's edges
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(src), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// every bulk store this thread issued has finished READING shared memory (the global writes may still be in flight)
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// this thread's generic-proxy shared-memory writes become visible to the async proxy (TMA)
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ uint4 ld_shared_v4(uint32_t addr) {
+  uint4 v;
+  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+  return v;
 }
 // 8-byte vector reduction (sm_90+): one RED for two fp32 adds
 __device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {
@@ -208,6 +228,14 @@ constexpr int A_STAGE_BYTES = 128 * 128;   // 128 rows x 128 B
 constexpr int B_STAGE_BYTES = 256 * 128;   // up to 256 rows x 128 B
 constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
 constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/ + 2048 /*column statistics*/;
+// form F: the ring, then the output staging area (two 16 KB slots, each one 128-row x 64-column 16-bit chunk of a
+// tile, 1024 B aligned for the 128B swizzle; the BatchNorm column statistics alias it, their launches store
+// directly), then the barriers
+constexpr int OUT_CHUNK_BYTES = 128 * 128;
+constexpr int OUT_STAGE_OFF = STAGES * STAGE_BYTES;
+constexpr int F_CTL_OFF = OUT_STAGE_OFF + 2 * OUT_CHUNK_BYTES;
+constexpr int F_SMEM_BYTES = F_CTL_OFF + 256 /*barriers*/ + 1024 /*align*/;
+static_assert(F_SMEM_BYTES <= 232448, "form-F shared memory exceeds the sm_90 opt-in limit");
 constexpr int NUM_THREADS = 384;           // producer warpgroup + two consumer warpgroups
 constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 
@@ -236,6 +264,7 @@ struct FTcParams {
   int out2_halo;             // reflect halo rows of out2 (its buffer has out_rows + 2 * out2_halo rows per batch element)
   const float* slope; int slope_mod;
   int bias_mask, slope_mask; // mod - 1 when the modulus is a power of two (the channel counts are), else -1
+  int tma_out;               // whole tiles leave through shared memory and TMA stores (16-bit out, no BatchNorm stats)
 };
 
 struct SharedCtl {
@@ -271,7 +300,8 @@ struct Piece {
 };
 
 // SEGAN_B200_DEBUG bit 20: phase timeline of tapgemm_f_tc (globaltimer ns; first consumer thread of every CTA):
-// [cta][0] = kernel start, then per piece: accumulator ready, epilogue done, (split tiles) finisher done; last = exit.
+// [cta][0] = kernel start, then per piece: accumulator ready, epilogue done (TMA-stored tiles: stores issued),
+// (split tiles) finisher done; last = exit.
 // Read back with sg_debug_timeline (diagnostics only).
 constexpr int TL_SLOTS = 32;
 constexpr int TL_CTAS = 160;
@@ -447,6 +477,108 @@ __device__ __forceinline__ void f_epilogue(const FTcParams& p, float (&acc)[TN /
   }
 }
 
+// Epilogue of a whole tile with a 16-bit `out` (every forward and data-gradient launch but fc.0 and BatchNorm-stat
+// launches), all 256 consumer threads together.  The tile leaves in 64-column chunks: the consumers write a chunk
+// into a 16 KB staging slot (rows in fragment order tb * TR + tr = the box's row order, 128B-swizzled so that the
+// 8 rows of one warp store hit different banks) and one thread writes the slot with a TMA tensor store whose box
+// {64, TR, TB} is clipped at the launch's columns, rows and batch elements.  Two slots: two chunks of `out` per
+// round, or a chunk of `out` and the same chunk of `out2`.  The stores of the last round drain while the consumers
+// run the next tile's MMAs; a slot is rewritten only after the issuing thread has seen its bulk group finish reading
+// (next round or next tile).  Per element the arithmetic is f_store2's: fp32 accumulator + bias, PReLU from fp32,
+// one rounding.  The reflect-halo mirror rows of out2 (rows reversed: no box expresses them) are copied from the
+// staged chunk with 16-byte stores.
+template <int TN>
+__device__ __forceinline__ void f_epilogue_tma(const FTcParams& p, const float (&acc)[TN / 2], int mt, int n0,
+                                               int ctid, uint32_t stg, const CUtensorMap* tmO,
+                                               const CUtensorMap* tmO2) {
+  const int lane = ctid & 31, cw = ctid >> 5;
+  const int mtb = p.m_tiles_per_b == 1 ? mt : mt / p.m_tiles_per_b;
+  const int b0 = mtb * p.TB;
+  const int m0 = p.m_lo + (mt - mtb * p.m_tiles_per_b) * p.TR;
+  const bool two = p.out2 != nullptr;
+  const bool act_in_place = p.slope != nullptr && !two;
+  const bool add_bias = p.bias != nullptr;
+  // this thread's 4-byte word of row cw * 16 + lane / 4 (+ 8 for h = 1, 1024 B further) in a staged chunk; the
+  // row's 16-byte column block jj sits at block jj ^ (row & 7) = jj ^ (lane / 4)
+  const uint32_t row_off = (uint32_t)(cw * 16 + (lane >> 2)) * 128u + 4u * (lane & 3);
+  const int sw = lane >> 2;
+  const int halo2 = p.out2_halo;
+  const bool mirror_tile = two && halo2 > 0 &&
+                           ((m0 <= halo2 && m0 + p.TR > 1) || (m0 + p.TR > p.out_rows - 1 - halo2 && m0 <= p.out_rows - 2));
+  constexpr int NQ = TN / 64;
+#pragma unroll
+  for (int q = 0; q < NQ; ++q) {
+    const bool round_start = two || (q & 1) == 0;
+    const bool round_end = two || (q & 1) == 1 || q == NQ - 1;
+    const uint32_t slot = stg + (two ? 0u : (uint32_t)(q & 1) * OUT_CHUNK_BYTES);
+    if (round_start) {
+      if (ctid == 0) bulk_wait_read_all();        // the slots' previous stores have read them ...
+      consumer_bar_sync();                        // ... before anyone writes them again
+    }
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      const int j = 8 * q + jj;
+      const int c = 8 * j + 2 * (lane & 3);
+      float bx = 0.f, by = 0.f;
+      if (add_bias) {    // bias_mod is a multiple of 64: no wrap inside the pair
+        const float* bp = p.bias + f_mod(n0 + c, p.bias_mod, p.bias_mask);
+        bx = __ldg(bp); by = __ldg(bp + 1);
+      }
+      float s0 = 0.f, s1 = 0.f;
+      if (p.slope != nullptr) {
+        const float* sp = p.slope + f_mod(n0 + c, p.slope_mod, p.slope_mask);
+        s0 = __ldg(sp); s1 = __ldg(sp + 1);
+      }
+      const uint32_t col_off = (uint32_t)((jj ^ sw) << 4);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float x = acc[4 * j + 2 * h] + bx, y = acc[4 * j + 2 * h + 1] + by;
+        if (act_in_place) {
+          x = x > 0.f ? x : s0 * x;
+          y = y > 0.f ? y : s1 * y;
+        }
+        const uint32_t off = row_off + (uint32_t)h * 1024u + col_off;
+        st_shared_u32(slot + off, pack2(x, y, p.out_dtype));
+        if (two) st_shared_u32(slot + OUT_CHUNK_BYTES + off, pack2(x > 0.f ? x : s0 * x, y > 0.f ? y : s1 * y, p.out_dtype));
+      }
+    }
+    if (!round_end) continue;
+    fence_proxy_async_smem();
+    consumer_bar_sync();
+    if (ctid == 0) {
+      const int c_rel = n0 - p.n_lo + 64 * q, m_rel = m0 - p.m_lo;
+      if (two) {
+        tma_store_3d(tmO, slot, c_rel, m_rel, b0);
+        tma_store_3d(tmO2, slot + OUT_CHUNK_BYTES, c_rel, m_rel, b0);
+      } else if (q & 1) {
+        tma_store_3d(tmO, stg, c_rel - 64, m_rel, b0);
+        tma_store_3d(tmO, stg + OUT_CHUNK_BYTES, c_rel, m_rel, b0);
+      } else {
+        tma_store_3d(tmO, stg, c_rel, m_rel, b0);
+      }
+      bulk_commit();
+    }
+    if (mirror_tile) {
+      // out2 rows m in [1, halo] also land on row -m, rows m in [out_rows-1-halo, out_rows-2] on 2(out_rows-1)-m
+      const int rows = p.TR * p.TB;
+      const int out2_buf_rows = p.out_rows + 2 * halo2;
+      for (int idx = ctid; idx < rows * 8; idx += 256) {
+        const int r = idx >> 3, k = idx & 7;
+        const int tb = r / p.TR, tr = r - tb * p.TR;
+        const int b = b0 + tb, m = m0 + tr;
+        if (b >= p.batch || m >= p.m_hi) continue;
+        int mm;
+        if (m >= 1 && m <= halo2) mm = -m;
+        else if (m >= p.out_rows - 1 - halo2 && m <= p.out_rows - 2) mm = 2 * (p.out_rows - 1) - m;
+        else continue;
+        const uint4 v = ld_shared_v4(slot + OUT_CHUNK_BYTES + (uint32_t)r * 128u + (uint32_t)((k ^ (r & 7)) << 4));
+        const int64_t o = ((int64_t)b * out2_buf_rows + halo2 + mm) * p.out_ld + p.out_col0 + (n0 - p.n_lo) + 64 * q + 8 * k;
+        *reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.out2) + o) = v;
+      }
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------
 // form F:  out[b,m,n] = bias + sum_d sum_kc A[b,m+d,kc] * Wp[d+4][n][kc]
 //   wgmma: M = 128 (rows: TB batches x TR rows; 64 per consumer warpgroup), N = TN output channels,
@@ -457,15 +589,20 @@ __device__ __forceinline__ void f_epilogue(const FTcParams& p, float (&acc)[TN /
 template <int TN, bool BF16>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 tapgemm_f_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
-             const __grid_constant__ CUtensorMap tmW, const FTcParams p) {
+             const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmO,
+             const __grid_constant__ CUtensorMap tmO2, const FTcParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  SharedCtl* ctl = reinterpret_cast<SharedCtl*>(smem + STAGES * STAGE_BYTES);
-  float* colstat = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES + 256);      // [2][256]
+  SharedCtl* ctl = reinterpret_cast<SharedCtl*>(smem + F_CTL_OFF);
+  float* colstat = reinterpret_cast<float*>(smem + OUT_STAGE_OFF);      // [2][256], aliases the output staging
   const int wg = threadIdx.x >> 7;
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmA0); prefetch_tmap(&tmA1); prefetch_tmap(&tmW);
+    if (p.tma_out) {
+      prefetch_tmap(&tmO);
+      if (p.out2 != nullptr) prefetch_tmap(&tmO2);
+    }
     for (int s = 0; s < STAGES; ++s) { mbar_init(&ctl->full[s], 1); mbar_init(&ctl->empty[s], 2); }
     fence_barrier_init();
   }
@@ -592,7 +729,8 @@ tapgemm_f_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ C
     if (tl_on && tl_i < TL_SLOTS - 1) tl[tl_i++] = gtime_ns();
 
     if (!partial) {
-      f_epilogue<TN>(p, acc, pc.mt, n0, ks, ctid, colstat);
+      if (p.tma_out) f_epilogue_tma<TN>(p, acc, pc.mt, n0, ctid, smem0 + OUT_STAGE_OFF, &tmO, &tmO2);
+      else f_epilogue<TN>(p, acc, pc.mt, n0, ks, ctid, colstat);
       if (tl_on && tl_i < TL_SLOTS - 1) tl[tl_i++] = gtime_ns();
       continue;
     }
@@ -631,6 +769,7 @@ tapgemm_f_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ C
   }
   if (tl_on && tl_i < TL_SLOTS) tl[tl_i++] = gtime_ns();
   if (p.stats != nullptr && stat_nt >= 0) flush_stats(stat_nt);
+  if (p.tma_out && ctid == 0) bulk_wait_read_all();   // shared memory outlives the last stores' reads
 }
 
 // ------------------------------------------------------------------------------------------
@@ -823,6 +962,29 @@ static int make_map2(CUtensorMap* m, const void* base, int dtype, int C, int64_t
   return SG_OK;
 }
 
+// 3-D store map over the columns [col0, col0 + C) and rows [row0, row0 + rows) of every batch element of a 16-bit
+// [B][buf_rows][ld] tensor, box (64, box_rows, box_b), 128B swizzle.  TMA needs 16-byte aligned bases and strides.
+static int make_store_map3(CUtensorMap* m, void* base, int dtype, int C, int rows, int B, int ld, int buf_rows,
+                           int row0, int col0, int box_rows, int box_b) {
+  EncodeTiledFn enc = get_encode();
+  if (!enc) { set_error("cuTensorMapEncodeTiled unavailable"); return SG_ERR_LAUNCH; }
+  uint8_t* p0 = reinterpret_cast<uint8_t*>(base) + ((int64_t)row0 * ld + col0) * 2;
+  SG_CHECK_ARG(ld % 8 == 0 && col0 % 8 == 0 && (reinterpret_cast<uintptr_t>(p0) & 15) == 0);
+  cuuint64_t dims[3] = {(cuuint64_t)C, (cuuint64_t)rows, (cuuint64_t)B};
+  cuuint64_t strides[2] = {(cuuint64_t)ld * 2, (cuuint64_t)ld * 2 * (cuuint64_t)buf_rows};
+  cuuint32_t box[3] = {64, (cuuint32_t)box_rows, (cuuint32_t)box_b};
+  cuuint32_t es[3] = {1, 1, 1};
+  CUresult r = enc(m, dtype == SG_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, p0, dims,
+                   strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                   CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeTiled(store C=%d rows=%d B=%d ld=%d box=%d,%d) failed: %d", C, rows, B, ld, box_rows,
+              box_b, (int)r);
+    return SG_ERR_LAUNCH;
+  }
+  return SG_OK;
+}
+
 // split-K workspace: counters [leftover tiles][8 consumer warps] u32 (8 KB), then one partial-sum slot per CTA
 // [SK_MAX_CTAS][128][256] fp32
 constexpr int SK_MAX_CTAS = 160;
@@ -935,10 +1097,30 @@ int tapgemm_f_tc_launch(const sg_tapgemm_f* q, cudaStream_t st) {
       p.sk_ws = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(q->sk_ws) + SK_CNT_BYTES);
     }
   }
+  // whole tiles of a 16-bit output leave through shared memory and TMA stores (f_epilogue_tma); fp32 outputs (atomic
+  // k-split, the waveform-end P), BatchNorm-stat launches and the split-K pieces store from the fragment
+  p.tma_out = q->out_dtype != SG_F32 && q->bn_stats == nullptr;
+  CUtensorMap tmO = tmA0, tmO2 = tmA0;
+  if (p.tma_out) {
+    rc = make_store_map3(&tmO, q->out, q->out_dtype, ncols, rows_m, q->batch, p.out_ld, q->out_rows + 2 * q->out_halo,
+                         q->out_halo + q->m_lo, p.out_col0, p.TR, p.TB);
+    if (rc) return rc;
+    if (q->out2 != nullptr) {
+      rc = make_store_map3(&tmO2, q->out2, q->out_dtype, ncols, rows_m, q->batch, p.out_ld,
+                           q->out_rows + 2 * q->out2_halo, q->out2_halo + q->m_lo, p.out_col0, p.TR, p.TB);
+      if (rc) return rc;
+    }
+  }
   const bool bf = q->a_dtype == SG_BF16;
-  if (p.TN == 256) return launch_persistent(bf ? tapgemm_f_tc<256, true> : tapgemm_f_tc<256, false>, nctas, tmA0, tmA1, tmW, &p, st);
-  if (p.TN == 128) return launch_persistent(bf ? tapgemm_f_tc<128, true> : tapgemm_f_tc<128, false>, nctas, tmA0, tmA1, tmW, &p, st);
-  return launch_persistent(bf ? tapgemm_f_tc<64, true> : tapgemm_f_tc<64, false>, nctas, tmA0, tmA1, tmW, &p, st);
+  void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, FTcParams);
+  if (p.TN == 256) kern = bf ? tapgemm_f_tc<256, true> : tapgemm_f_tc<256, false>;
+  else if (p.TN == 128) kern = bf ? tapgemm_f_tc<128, true> : tapgemm_f_tc<128, false>;
+  else kern = bf ? tapgemm_f_tc<64, true> : tapgemm_f_tc<64, false>;
+  SG_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, F_SMEM_BYTES));
+  void* args[] = {&tmA0, &tmA1, &tmW, &tmO, &tmO2, &p};
+  SG_CHECK_CUDA(cudaLaunchKernel(reinterpret_cast<const void*>(kern), dim3(nctas), dim3(NUM_THREADS), args,
+                                 (size_t)F_SMEM_BYTES, st));
+  return SG_OK;
 }
 
 template <typename K>

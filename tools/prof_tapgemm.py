@@ -1,6 +1,8 @@
-"""Launches representative SEGAN+ layer shapes of the two tensor-core tap-GEMMs at batch 300 (for ncu /
-timing): conv fwd enc2 (Cin 128 -> 256), deconv fwd dec1 (1024 -> 256, two K sources), conv dgrad enc3,
-wgrad enc2, wgrad dec1.  Prints CUDA-event times and TFLOP/s."""
+"""Launches representative SEGAN+ layer shapes of the two tensor-core tap-GEMMs at batch 300 (for timing): conv
+forward and data gradient of every encoder level, the decoder deconvs (two K sources), the weight gradients, the
+Generator's fused PReLU + reflect-halo outputs (out2) and the waveform-end single-tap GEMMs.  Prints CUDA-event times
+and TFLOP/s.  `one <names>` runs single shapes; with SEGAN_B200_DEBUG=1048576 it also prints each one's per-CTA
+phase timeline."""
 import os
 import sys
 
@@ -53,25 +55,42 @@ def timeit(name, fn, flops):
                                           for i, ms in enumerate(res))))
 
 
-def conv_fwd(cin, cout, R):
+def _out2(rows, cols, halo):
+    """The Generator blocks' fused second output: PReLU(out) with a reflect halo (sg_tapgemm_f.out2)."""
+    if halo is None:
+        return {}
+    return dict(out2=torch.empty(B, rows + 2 * halo, cols, device=dev, dtype=torch.float16), out2_halo=halo,
+                slope=torch.rand(cols, device=dev) * 0.3, slope_mod=cols)
+
+
+def conv_fwd(cin, cout, R, out2_halo=None):
+    """out2_halo: None = the Discriminator's conv (one output), else the Generator's encoder block with its out2."""
     a = h(B, R + 8, 4 * cin)
     w = h(9, cout, 4 * cin)
     out = torch.empty(B, R, cout, device=dev, dtype=torch.float16)
+    bias = torch.randn(cout, device=dev)
     taps = E.tap_ranges("conv_fwd", cin, 4 * cin, cout)
     fl = E._tap_flops(taps, -4, 4, 0, cout, R * B)
-    timeit("conv_fwd %d->%d R=%d" % (cin, cout, R),
-           lambda: E.run_f(a, None, R, 4, SG_F16, w, SG_F16, 4 * cin, cout, taps, out, SG_F16, R, 0, 0, R, B, backend=1), fl)
+    kw = _out2(R, cout, out2_halo)
+    timeit("conv_fwd %d->%d R=%d%s" % (cin, cout, R, "" if out2_halo is None else " out2 halo %d" % out2_halo),
+           lambda: E.run_f(a, None, R, 4, SG_F16, w, SG_F16, 4 * cin, cout, taps, out, SG_F16, R, 0, 0, R, B,
+                           bias=bias, bias_mod=cout, backend=1, **kw), fl)
 
 
-def deconv_fwd(cin, cout, R):
+def deconv_fwd(cin, cout, R, out2=False):
+    """out2: the Generator's decoder block as the train step runs it (raw output + PReLU output, no halo)."""
     a0, a1 = h(B, R, cin // 2), h(B, R, cin // 2)
     w = h(9, 4 * cout, cin)
     out = torch.empty(B, R, 4 * cout, device=dev, dtype=torch.float16)
+    bias = torch.randn(cout, device=dev)
     taps = E.tap_ranges("deconv_fwd", cout, cin, 4 * cout)
     fl = E._tap_flops(taps, -4, 4, 0, 4 * cout, R * B)
-    timeit("deconv_fwd %d->%d R=%d" % (cin, cout, R),
+    kw = _out2(R, 4 * cout, 0 if out2 else None)
+    if out2:
+        kw["slope_mod"] = cout
+    timeit("deconv_fwd %d->%d R=%d%s" % (cin, cout, R, " out2" if out2 else ""),
            lambda: E.run_f(a0, a1, R, 0, SG_F16, w, SG_F16, cin, 4 * cout, taps, out, SG_F16, R, 0, 0, R, B,
-                           a0_c=cin // 2, a1_c=cin // 2, backend=1), fl)
+                           bias=bias, bias_mod=cout, a0_c=cin // 2, a1_c=cin // 2, backend=1, **kw), fl)
 
 
 def conv_dgrad(cin, cout, R):
@@ -97,17 +116,19 @@ def conv_wgrad(cin, cout, R):
            lambda: E.run_w(g, R, SG_BF16, a, None, R, 4, SG_BF16, 4 * cin, cout, taps, dw, B, ksplit=ks, backend=1), fl)
 
 
-def wave0():
-    """The waveform-end layer as it runs in the step: single-tap GEMM over the 64-column im2col (K = 64, N = 64)."""
+def wave0(out2_halo=None):
+    """The waveform-end layer as it runs in the step: single-tap GEMM over the 64-column im2col (K = 64, N = 64).
+    out2_halo None: the Discriminator's enc0 (one output); 16: the Generator's enc0 with its fused out2."""
     col = h(B, 4096, 64)
     w = h(1, 64, 64)
     bias = torch.randn(64, device=dev)
     out = torch.empty(B, 4096, 64, device=dev, dtype=torch.float16)
     taps = E.tap_ranges("full", 0, 64, 64)
     fl = 2.0 * B * 4096 * 64 * 64
-    timeit("wave0 im2col-GEMM 64x64 R=4096", lambda: E.run_f(col, None, 4096, 0, SG_F16, w, SG_F16, 64, 64, taps, out,
-                                                              SG_F16, 4096, 0, 0, 4096, B, bias=bias, bias_mod=64,
-                                                              d_lo=0, d_hi=0, w_tap0=4, backend=1), fl)
+    kw = _out2(4096, 64, out2_halo)
+    timeit("wave0 im2col-GEMM 64x64 R=4096%s" % ("" if out2_halo is None else " out2 halo %d" % out2_halo),
+           lambda: E.run_f(col, None, 4096, 0, SG_F16, w, SG_F16, 64, 64, taps, out, SG_F16, 4096, 0, 0, 4096, B,
+                           bias=bias, bias_mod=64, d_lo=0, d_hi=0, w_tap0=4, backend=1, **kw), fl)
 
 
 def dump_timeline(name):
@@ -140,7 +161,9 @@ def dump_timeline(name):
     print("exit times us: min %.1f median %.1f max %.1f" % (ends[0], ends[len(ends) // 2], ends[-1]))
 
 
-ONE = {"wave0": wave0, "enc1": lambda: conv_fwd(64, 128, 1024), "enc3": lambda: conv_fwd(256, 512, 64),
+ONE = {"wave0": wave0, "denc0": wave0, "genc0": lambda: wave0(16),
+       "enc1": lambda: conv_fwd(64, 128, 1024), "genc1": lambda: conv_fwd(64, 128, 1024, 16),
+       "enc3": lambda: conv_fwd(256, 512, 64), "gdec1": lambda: deconv_fwd(1024, 256, 64, out2=True),
        "enc4": lambda: conv_fwd(512, 1024, 16), "dec1": lambda: deconv_fwd(1024, 256, 64),
        "dgrad3": lambda: conv_dgrad(256, 512, 64), "wgrad3": lambda: conv_wgrad(256, 512, 64),
        "wgrad4": lambda: conv_wgrad(512, 1024, 16)}
@@ -160,17 +183,15 @@ if __name__ == "__main__":
                          (conv_dgrad, (256, 512, 64)), (conv_dgrad, (128, 256, 256)), (conv_dgrad, (64, 128, 1024))):
             fn(*args)
         sys.exit(0)
-    if COMPARE == "areuse3":          # three representative shapes only (timing experiments)
-        COMPARE = "areuse"
-        conv_fwd(64, 128, 1024)
-        deconv_fwd(512, 128, 256)
-        conv_dgrad(128, 256, 256)
-        sys.exit(0)
+    wave0()
+    wave0(16)
     conv_fwd(64, 128, 1024)
+    conv_fwd(64, 128, 1024, 16)
     conv_fwd(128, 256, 256)
     conv_fwd(256, 512, 64)
     conv_fwd(512, 1024, 16)
     deconv_fwd(2048, 512, 16)
+    deconv_fwd(1024, 256, 64, out2=True)
     deconv_fwd(1024, 256, 64)
     deconv_fwd(512, 128, 256)
     deconv_fwd(256, 64, 1024)
