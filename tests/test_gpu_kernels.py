@@ -67,13 +67,11 @@ def _restore_cta_pair():
         _lib.load().sg_set_ew_variant(kind, *v)
 
 
-@pytest.mark.parametrize("backend", [BACKEND_FFMA, BACKEND_TCGEN05, 2])
-@pytest.mark.parametrize("case", ["conv_fwd", "conv_dgrad", "deconv_fwd_cat", "deconv_dgrad", "small_rows", "fc"])
-def test_tapgemm_f(backend, case):
-    """backend 1 = tensor cores with sg_set_cta_pair(0), 2 = tensor cores with sg_set_cta_pair(1)."""
-    _lib.load().sg_set_cta_pair(1 if backend == 2 else 0)
-    if backend == 2:
-        backend = BACKEND_TCGEN05
+F_CASES = ["conv_fwd", "conv_dgrad", "deconv_fwd_cat", "deconv_dgrad", "small_rows", "fc"]
+
+
+def _f_case(case):
+    """The operands and geometry of one test_tapgemm_f case, as a dict of its local names."""
     g = _gen(1)
     B = 3
     bias = None
@@ -133,6 +131,22 @@ def test_tapgemm_f(backend, case):
         d_lo = d_hi = 0
         w_tap0, ksplit = 4, 4
         adt, wdt, out_dtype, tdt = SG_F16, SG_F16, SG_F32, torch.float32
+    return dict(locals())
+
+
+@pytest.mark.parametrize("backend", [BACKEND_FFMA, BACKEND_TCGEN05, 2])
+@pytest.mark.parametrize("case", F_CASES)
+def test_tapgemm_f(backend, case):
+    """backend 1 = tensor cores with sg_set_cta_pair(0), 2 = tensor cores with sg_set_cta_pair(1)."""
+    _lib.load().sg_set_cta_pair(1 if backend == 2 else 0)
+    if backend == 2:
+        backend = BACKEND_TCGEN05
+    c = _f_case(case)
+    B, R, halo, kc, nc, taps, w, a0, a1, a1_c, bias = (c[k] for k in ("B", "R", "halo", "kc", "nc", "taps", "w", "a0", "a1",
+                                                                       "a1_c", "bias"))
+    m_lo, m_hi, out_rows, out_halo, n_lo, n_hi = (c[k] for k in ("m_lo", "m_hi", "out_rows", "out_halo", "n_lo", "n_hi"))
+    d_lo, d_hi, w_tap0, ksplit = (c[k] for k in ("d_lo", "d_hi", "w_tap0", "ksplit"))
+    adt, wdt, out_dtype, tdt = (c[k] for k in ("adt", "wdt", "out_dtype", "tdt"))
     nhi = nc if n_hi is None else n_hi
     out = torch.zeros(B, out_rows + 2 * out_halo, nc, dtype=tdt, device=DEV)
     E.run_f(a0, a1, R, halo, adt, w, wdt, kc, nc, taps, out, out_dtype, out_rows, out_halo, m_lo, m_hi, B,
@@ -153,12 +167,11 @@ def test_tapgemm_f(backend, case):
         assert float(out[:, :, :n_lo].abs().max()) == 0.0
 
 
-@pytest.mark.parametrize("case", ["conv_fwd", "conv_fwd_n512", "deconv_cat", "conv_dgrad_halo", "deconv_dgrad_sub", "taps3"])
-def test_tapgemm_f_a_reuse(case):
-    """sg_set_cta_pair(2) (the activation-reuse schedule's setting; the sm_90a kernels run one schedule for every
-    setting).  Shapes with >= 128 rows per batch element,
-    a partial last M tile, an odd number of M tiles, two K sources, halo'd outputs and N sub-ranges."""
-    _lib.load().sg_set_cta_pair(2)
+F_REUSE_CASES = ["conv_fwd", "conv_fwd_n512", "deconv_cat", "conv_dgrad_halo", "deconv_dgrad_sub", "taps3"]
+
+
+def _f_reuse_case(case):
+    """The operands and geometry of one test_tapgemm_f_a_reuse case, as a dict of its local names."""
     g = _gen(8)
     B = 5
     a1, a1_c, bias = None, 0, None
@@ -197,6 +210,20 @@ def test_tapgemm_f_a_reuse(case):
         m_lo, m_hi, out_rows, out_halo = 0, R, R, 0
         n_lo, n_hi = 256, 512
         adt, odt, tdt = SG_BF16, SG_BF16, torch.bfloat16
+    return dict(locals())
+
+
+@pytest.mark.parametrize("case", F_REUSE_CASES)
+def test_tapgemm_f_a_reuse(case):
+    """sg_set_cta_pair(2) (the activation-reuse schedule's setting; the sm_90a kernels run one schedule for every
+    setting).  Shapes with >= 128 rows per batch element,
+    a partial last M tile, an odd number of M tiles, two K sources, halo'd outputs and N sub-ranges."""
+    _lib.load().sg_set_cta_pair(2)
+    c = _f_reuse_case(case)
+    B, R, halo, kc, nc, taps, w, a0, a1, a1_c, bias = (c[k] for k in ("B", "R", "halo", "kc", "nc", "taps", "w", "a0", "a1",
+                                                                       "a1_c", "bias"))
+    m_lo, m_hi, out_rows, out_halo, n_lo, n_hi = (c[k] for k in ("m_lo", "m_hi", "out_rows", "out_halo", "n_lo", "n_hi"))
+    d_lo, d_hi, adt, odt, tdt = (c[k] for k in ("d_lo", "d_hi", "adt", "odt", "tdt"))
     nhi = nc if n_hi is None else n_hi
     out = torch.zeros(B, out_rows + 2 * out_halo, nc, dtype=tdt, device=DEV)
     E.run_f(a0, a1, R, halo, adt, w, adt, kc, nc, taps, out, odt, out_rows, out_halo, m_lo, m_hi, B,
