@@ -85,17 +85,13 @@ __device__ __forceinline__ void unpack8(const U4& x, bool f16, float (&v)[8]) {
     v[2 * i] = f.x; v[2 * i + 1] = f.y;
   }
 }
-__device__ __forceinline__ uint4 pack8(const float (&v)[8], bool f16, bool sat) {
+// fp16 stores saturate at +-65504 (as in elementwise.cu and the tap-GEMM epilogue): every variant stores the same bits
+__device__ __forceinline__ uint4 pack8(const float (&v)[8], bool f16) {
   uint32_t w[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     if (f16) {
-      if (sat) {
-        w[i] = pack_half2_sat(v[2 * i], v[2 * i + 1]);
-      } else {
-        __half2 h2 = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
-        w[i] = *reinterpret_cast<uint32_t*>(&h2);
-      }
+      w[i] = pack_half2_sat(v[2 * i], v[2 * i + 1]);
     } else {
       __nv_bfloat162 h2 = __floats2bfloat162_rn(v[2 * i], v[2 * i + 1]);
       w[i] = *reinterpret_cast<uint32_t*>(&h2);
@@ -346,7 +342,7 @@ act_bwd_bulk_kernel(const SeBwd p) {
           for (int j = 0; j < 8; ++j) out[j] = fmaf(so[j], g[j], fmaf(ka[j], x[j], kb[j]));
         }
         if (p.g_a_out)
-          *reinterpret_cast<uint4*>(p.g_a_out + ((int64_t)tw.b * L + l0 + r) * C + c0) = pack8(out, gf16, true);
+          *reinterpret_cast<uint4*>(p.g_a_out + ((int64_t)tw.b * L + l0 + r) * C + c0) = pack8(out, gf16);
       }
     }
     __syncwarp();
@@ -531,7 +527,7 @@ act_fwd_bulk_kernel(const uint16_t* __restrict__ a, int a_f16, int batch, int L,
           if (prelu) y = y > 0.f ? y : sl[j] * y;
           x[j] = y;
         }
-        const uint4 o = pack8(x, f16, false);
+        const uint4 o = pack8(x, f16);
         const int q = qs + r;
         *reinterpret_cast<uint4*>(hb + (int64_t)q * C) = o;
         if (H > 0) {
