@@ -126,14 +126,18 @@ typedef struct sg_tapgemm_f {
   /* per tap (index d+4): valid K range [k_lo, k_hi) and valid N range [n_lo, n_hi) in channels
      (multiples of 64); blocks outside are structurally zero in Wp and are skipped */
   int32_t tap_k_lo[9], tap_k_hi[9], tap_n_lo[9], tap_n_hi[9];
-  void* out;          /* [B][out_halo + out_rows + out_halo][out_ld]; column of channel n = n - n_lo + out_col0 */
+  void* out;          /* [B][out_halo + out_rows + out_halo][out_ld]; column of channel n = n - n_lo + out_col0
+                         (out_ld <= 0: out_ld = nc, out_col0 = n_lo); out_col0 + (n_hi - n_lo) <= out_ld */
   int32_t out_ld, out_col0;
-  int32_t out_dtype;  /* SG_F16 | SG_BF16 | SG_F32 (F32: atomically accumulated, pre-zeroed by caller) */
+  int32_t out_dtype;  /* SG_F16 | SG_BF16 | SG_F32.  F32 with ksplit = 1 overwrites the destination; with ksplit > 1
+                         the splits are atomically accumulated into it (the caller prepares it, e.g. zeroes it).
+                         Column pairs are stored together: out_ld and out_col0 even, out aligned to two elements.
+                         fp16 stores saturate at +-65504 */
   int32_t out_rows, out_halo;
   int32_t m_lo, m_hi; /* rows computed per batch element (may reach into the out halo) */
   int32_t n_lo, n_hi; /* channels computed */
   const float* bias;  /* or NULL */
-  int32_t bias_mod;   /* bias index = n % bias_mod */
+  int32_t bias_mod;   /* bias index = n % bias_mod; a multiple of 64 (<= 0: nc) */
   int32_t batch;
   int32_t ksplit;     /* >1 only with out_dtype == SG_F32 */
   int32_t backend;    /* SG_BACKEND_* */

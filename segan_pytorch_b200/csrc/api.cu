@@ -89,6 +89,16 @@ extern "C" int sg_tapgemm_f_run(const sg_tapgemm_f* p, void* stream) {
   SG_CHECK_ARG(p->ksplit <= 1 || p->out_dtype == SG_F32);
   SG_CHECK_ARG(p->m_lo >= -p->out_halo && p->m_hi <= p->out_rows + p->out_halo && p->m_lo < p->m_hi);
   SG_CHECK_ARG(p->batch > 0 && p->a_rows > 0 && p->a_halo >= 0);
+  {
+    // the launch's columns stay inside one row of `out`; column pairs are stored together (half2 / float2 / red.v2)
+    const int ld = p->out_ld > 0 ? p->out_ld : p->nc, col0 = p->out_ld > 0 ? p->out_col0 : p->n_lo;
+    const uintptr_t pair = p->out_dtype == SG_F32 ? 8 : 4;
+    SG_CHECK_ARG(col0 >= 0 && col0 + (p->n_hi - p->n_lo) <= ld);
+    SG_CHECK_ARG(ld % 2 == 0 && col0 % 2 == 0 && reinterpret_cast<uintptr_t>(p->out) % pair == 0);
+    SG_CHECK_ARG(p->out2 == nullptr || reinterpret_cast<uintptr_t>(p->out2) % pair == 0);
+  }
+  // bias pairs are read without a wrap inside the pair
+  SG_CHECK_ARG(p->bias == nullptr || p->bias_mod <= 0 || p->bias_mod % 64 == 0);
   if (p->out2 != nullptr || p->slope != nullptr) {
     SG_CHECK_ARG(p->slope != nullptr && p->slope_mod > 0 && p->slope_mod % 64 == 0 && p->out_dtype != SG_F32);
     SG_CHECK_ARG(p->ksplit <= 1 && p->out2_halo >= 0);

@@ -93,8 +93,17 @@ __global__ void __launch_bounds__(256) tapgemm_f_ffma(FParams p) {
       float v = acc[i][j];
       if (p.bias && ks == 0) v += p.bias[n % p.bias_mod];
       const int64_t o = ((int64_t)b * out_buf_rows + (m + p.out_halo)) * p.out_ld + (n - p.n_lo + p.out_col0);
-      if (p.out_dtype == SG_F32) atomicAdd(reinterpret_cast<float*>(p.out) + o, v);
-      else st16(p.out, o, v, p.out_dtype);
+      // fp32: an interleaved k-split (ksplit > 1) accumulates into the caller's destination, ksplit = 1 overwrites
+      // it (as the tensor-core epilogue does); fp16 saturates at +-65504 like the tensor-core stores
+      if (p.out_dtype == SG_F32) {
+        float* dst = reinterpret_cast<float*>(p.out) + o;
+        if (p.ksplit > 1) atomicAdd(dst, v);
+        else *dst = v;
+      } else if (p.out_dtype == SG_F16) {
+        reinterpret_cast<uint16_t*>(p.out)[o] = (uint16_t)(pack_half2_sat(v, 0.f) & 0xffffu);
+      } else {
+        st16(p.out, o, v, p.out_dtype);
+      }
     }
   }
 }

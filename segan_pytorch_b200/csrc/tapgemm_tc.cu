@@ -354,7 +354,9 @@ struct PieceIter {
     pc.total = s;
     pc.kb = (int)((long long)s * part / p.sk_split);
     pc.ke = (int)((long long)s * (part + 1) / p.sk_split);
-    return pc.kb < pc.ke;
+    // an empty piece (a tile with fewer k-steps than sk_split: its N range misses some taps) still runs: it stores a
+    // zero partial and counts, otherwise the tile is never finished and its counter is left non-zero
+    return true;
   }
 };
 
@@ -703,7 +705,7 @@ tapgemm_f_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ C
     const int ks = p.ksplit == 1 ? 0 : pc.rest % p.ksplit;
     const int nt = p.ksplit == 1 ? pc.rest : pc.rest / p.ksplit;
     const int n0 = p.n_lo + nt * p.TN;
-    const bool partial = pc.kb != 0 || pc.ke != pc.total;         // one K range of a split tile
+    const bool partial = pc.tile >= it.dp_end;                     // one K range (possibly empty) of a split tile
     if (p.stats != nullptr && nt != stat_nt) {
       if (stat_nt >= 0) flush_stats(stat_nt);
       stat_nt = nt;

@@ -54,7 +54,7 @@ def ref_w(g, a0, a1, a_halo, taps, d_lo=-4, d_hi=4):
 
 def ref_f(a0, a1, a_halo, w, taps, m_lo, m_hi, d_lo=-4, d_hi=4, w_tap0=0, bias=None):
     """(ref, mag), float64 [B][m_hi - m_lo][nc] on a0's device.  w [slots][nc][kc]; only each tap's live box of it
-    is read."""
+    is read.  bias [bias_mod]: channel n adds bias[n % bias_mod]."""
     a = _cat(a0, a1)
     B, nc = a.shape[0], w.shape[1]
     rows = m_hi - m_lo
@@ -68,7 +68,7 @@ def ref_f(a0, a1, a_halo, w, taps, m_lo, m_hi, d_lo=-4, d_hi=4, w_tap0=0, bias=N
         ref[..., n0:n1] += A @ Wt
         mag[..., n0:n1] += A.abs() @ Wt.abs()
     if bias is not None:
-        b = bias.double().repeat(nc // bias.numel())
+        b = bias.double()[torch.arange(nc, device=bias.device) % bias.numel()]
         ref += b
         mag += b.abs()
     return ref, mag
@@ -76,7 +76,7 @@ def ref_f(a0, a1, a_halo, w, taps, m_lo, m_hi, d_lo=-4, d_hi=4, w_tap0=0, bias=N
 
 def prelu_ref(ref, mag, slope):
     """PReLU applied to the fp32 value before the one rounding: (act, mag_act).  slope [slope_mod] repeats over n."""
-    s = slope.double().repeat(ref.shape[-1] // slope.numel())
+    s = slope.double()[torch.arange(ref.shape[-1], device=slope.device) % slope.numel()]
     act = torch.where(ref > 0, ref, ref * s)
     return act, torch.where(ref > 0, mag, mag * s.abs() + act.abs())
 
@@ -113,8 +113,27 @@ def half_ulp(v, fmt):
     return torch.ldexp(torch.ones_like(v, dtype=torch.float64), e - p - 1)
 
 
-def c_f(got16, ref, mag, fmt):
-    """The error of a 16-bit store in excess of half an output ulp, over U * mag.  fp16 stores saturate at +-65504."""
+def c_f(got16, ref, mag, fmt, trunc_stages=0):
+    """The error of a 16-bit store in excess of half an output ulp, over U * mag.  fp16 stores saturate at +-65504.
+    trunc_stages: as in c_w (the same accumulator), a number or a tensor that broadcasts against ref (per column)."""
     tgt = ref.clamp(-65504.0, 65504.0) if fmt == "f16" else ref
     err = (got16.double() - tgt).abs() - half_ulp(tgt, fmt)
-    return _ratio(err.clamp_min(0.0), U * mag)
+    return _ratio(err.clamp_min(0.0), U * mag * (1.0 + TRUNC_PER_STAGE * trunc_stages))
+
+
+def c_pair(got_a, got_b, mag, fmt=None, trunc_stages=0):
+    """Distance between two results of the same launch in the units of c_f / c_w: each may be off the fp64 value by
+    C_TOL (and, stored in a 16-bit format, by half an ulp of itself), so two correct ones stay within 2 C_TOL."""
+    err = (got_a.double() - got_b.double()).abs()
+    if fmt is not None:
+        err = (err - half_ulp(got_a, fmt) - half_ulp(got_b, fmt)).clamp_min(0.0)
+    return _ratio(err, U * mag * (1.0 + TRUNC_PER_STAGE * trunc_stages))
+
+
+def f_stages(taps, d_lo, d_hi, n0, n1, split=1):
+    """64-channel k-steps one form-F tensor-core accumulator walks for the tile of columns [n0, n1): every live tap
+    whose N range overlaps the tile contributes its K range; a tile split `split` ways (stream-K pieces, interleaved
+    fp32 k-split) gives each piece at most ceil(steps / split), and the pieces are added in fp32 with rounding."""
+    steps = sum((taps[1][d + 4] - taps[0][d + 4]) // 64 for d in range(d_lo, d_hi + 1)
+                if taps[2][d + 4] < n1 and taps[3][d + 4] > n0)
+    return -(-steps // max(1, split))

@@ -138,7 +138,7 @@ def test_tapgemm_f_stream_k_cases_vs_fp64(case, stream_k):
         torch.cuda.synchronize()
     finally:
         E.STREAM_K = prev
-        lib.sg_set_stream_k(16, 2.5)
+        lib.sg_set_stream_k(16, 4.5)             # the default cost model
     assert (int(ws[8192:].count_nonzero()) > 0) == stream_k
     ref, mag = M.ref_f(a0, None, halo, w, taps, m_lo, m_hi, bias=bias)
     _gate("stream_k=%s %s" % (stream_k, case), out[:, out_halo + m_lo:out_halo + m_hi], ref, mag, "f16")

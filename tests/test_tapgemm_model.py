@@ -26,7 +26,12 @@ So at the magnitudes they draw, the old gates do see an index error that moves w
 see is anything below 2e-3 / 3e-2 absolute -- a loss of accumulation precision three orders above the arithmetic's
 own error, any defect on small values (their floor max(1, .) is absolute, c is scale-free), a stray accumulation
 outside the live ranges -- and they never launch out_scale with the production format.  The clean emulation sits at
-c < 7."""
+c < 7.
+
+The paths tests/test_gpu_tapgemm_f.py adds have their own planted defects, each far outside the gate: a row read from
+the neighbouring packed batch element instead of the zero fill (3.9e6), an out2 reflect-halo row mirrored one row
+off (1.3e9), a bias modulus of 192 applied as a mask (3.1e7), a stream-K finisher that drops one of four partial sums
+(1.3e6).  c_f takes the same per-stage truncation allowance as c_w."""
 import pytest
 import torch
 
@@ -270,6 +275,123 @@ def test_f_planted_error_fails_the_gate(name):
           % (name, c, *("passes" if o else "fails" for o in old)))
     assert c > 20 * M.C_TOL
     assert old == F_PLANTED[name]
+
+
+# ------------------------------------------------------------------------------------------------------
+# form F defects of the packed-row, fused-epilogue and stream-K paths (tests/test_gpu_tapgemm_f.py's gate)
+# ------------------------------------------------------------------------------------------------------
+def _f_steps():
+    return [(d, k0) for d in range(-4, 5) for k0 in range(TAPS[0][d + 4], TAPS[1][d + 4], 64)]
+
+
+def _f_acc(a, halo, w, steps, wrong_batch=None):
+    """fp32 sum over the given (tap, 64-channel block) steps.  wrong_batch = (tap, b, m): row m + d lies past the
+    end of batch element b's buffer (halo 0), and is read from the next packed batch element instead of as zero."""
+    acc = torch.zeros(a.shape[0], FR, NC)
+    for d, k0 in steps:
+        rows = M.shifted_rows(a, halo, d, FR)[..., k0:k0 + 64].float()
+        if wrong_batch is not None and d == wrong_batch[0]:
+            _, b, m = wrong_batch
+            assert m + d >= FR
+            rows[b, m] = a[b + 1, m + d - FR, k0:k0 + 64].float()
+        acc += rows @ w[d + 4, :, k0:k0 + 64].float().t()
+    return acc
+
+
+def test_f_truncation_allowance_applies_to_c_f():
+    """A 16-bit result 100 U * mag beyond half an ulp (a 300-stage sum that shrank by a third of U * mag per stage)
+    passes with the stages declared (a number or one per column) and fails without."""
+    got = torch.tensor([[1000.0, -1000.0]]).to(torch.bfloat16)
+    mag = torch.tensor([[4000.0, 4000.0]], dtype=torch.float64)
+    ref = got.double() + got.double().sign() * (M.half_ulp(got, "bf16") + 100 * M.U * mag)
+    assert M.c_f(got, ref, mag, "bf16") == pytest.approx(100.0)
+    assert M.c_f(got, ref, mag, "bf16", 300) <= M.C_TOL
+    assert M.c_f(got, ref, mag, "bf16", torch.tensor([300.0, 300.0], dtype=torch.float64)) <= M.C_TOL
+    assert M.c_f(got, ref, mag, "bf16", torch.tensor([300.0, 0.0], dtype=torch.float64)) > M.C_TOL
+
+
+def test_f_stages_counts_the_taps_a_tile_reaches():
+    assert M.f_stages(TAPS, -4, 4, 0, 128) == 31                 # 7 whole taps x 4 + 2 + 1
+    assert M.f_stages(TAPS, -4, 4, 0, 128, split=2) == 16
+    assert M.f_stages(TAPS, -4, -4, 0, 128) == 2
+    dg = ([0] * 9, [256] * 9, [0] * 9, [512] * 9)
+    dg[3][0] = 128                                               # tap -4 reaches columns 0..128 only
+    assert M.f_stages(dg, -4, -3, 0, 256) == 8 and M.f_stages(dg, -4, -3, 256, 512) == 4
+
+
+def test_f_planted_neighbouring_batch_row_fails_the_gate():
+    """No halo, +-64 in the first and last row of every batch element: tap +1 of the last row of element 0 reads
+    element 1's first row instead of the zero fill."""
+    g = _gen(15)
+    a, w, bias = _f_problem()
+    a = torch.randn(FB, FR, KC, generator=g)
+    a[:, 0] = torch.where(torch.rand(FB, KC, generator=g) < 0.5, -64.0, 64.0)
+    a[:, -1] = torch.where(torch.rand(FB, KC, generator=g) < 0.5, -64.0, 64.0)
+    a = a.half()
+    ref, mag = M.ref_f(a, None, 0, w, TAPS, 0, FR, bias=bias)
+    clean = (_f_acc(a, 0, w, _f_steps()) + bias).half()
+    assert M.c_f(clean, ref, mag, "f16") <= M.C_TOL / 4
+    got = (_f_acc(a, 0, w, _f_steps(), wrong_batch=(1, 0, FR - 1)) + bias).half()
+    c = M.c_f(got, ref, mag, "f16")
+    print("form F planted next_batch_element_row: c = %.3g" % c)
+    assert c > 20 * M.C_TOL
+
+
+def test_f_planted_out2_mirror_row_off_by_one_fails_the_gate():
+    """out2 with a reflect halo of 4: row -m is PReLU(out row m); the planted kernel copies row m + 1."""
+    a, w, bias = _f_problem()
+    slope = 0.3 * torch.rand(NC, generator=_gen(16))
+    ref, mag = M.ref_f(a, None, FH, w, TAPS, 0, FR, bias=bias)
+    act, mag_act = M.prelu_ref(ref, mag, slope)
+    acc = _f_acc(a, FH, w, _f_steps()) + bias
+    out2 = torch.where(acc > 0, acc, acc * slope).half()
+    h = 4
+    want, want_mag = act[:, 1:h + 1].flip(1), mag_act[:, 1:h + 1].flip(1)       # halo rows -h .. -1
+    safe = M.sign_safe(ref[:, 1:h + 1].flip(1), mag[:, 1:h + 1].flip(1))
+    good = out2[:, 1:h + 1].flip(1)
+    assert M.c_f(good[safe], want[safe], want_mag[safe], "f16") <= M.C_TOL / 4
+    bad = out2[:, 2:h + 2].flip(1)
+    c = M.c_f(bad[safe], want[safe], want_mag[safe], "f16")
+    print("form F planted out2_mirror_off_by_one: c = %.3g" % c)
+    assert c > 20 * M.C_TOL
+
+
+def test_f_planted_bias_mod_as_a_mask_fails_the_gate():
+    """bias_mod = 192 over 384 channels: n & 191 is not n % 192 (n = 64 reads bias[0])."""
+    g = _gen(17)
+    nc, mod = 384, 192
+    a = torch.randn(2, 32, 64, generator=g).half()
+    w = (0.05 * torch.randn(1, nc, 64, generator=g)).half()
+    bias = torch.randn(mod, generator=g)
+    taps = ([0] * 9, [64] * 9, [0] * 9, [nc] * 9)
+    ref, mag = M.ref_f(a, None, 0, w, taps, 0, 32, 0, 0, 4, bias)
+    acc = a.float() @ w[0].float().t()
+    n = torch.arange(nc)
+    clean = (acc + bias[n % mod]).half()
+    assert M.c_f(clean, ref, mag, "f16") <= M.C_TOL / 4
+    got = (acc + bias[n & (mod - 1)]).half()
+    c = M.c_f(got, ref, mag, "f16")
+    print("form F planted bias_mod_as_mask: c = %.3g" % c)
+    assert c > 20 * M.C_TOL
+
+
+def test_f_planted_finisher_dropping_a_partial_fails_the_gate():
+    """Stream-K: the 31 k-steps split over 4 pieces, their fp32 partial sums added in slot order by the finisher;
+    the planted finisher adds 3 of the 4 slots."""
+    a, w, bias = _f_problem()
+    ref, mag = M.ref_f(a, None, FH, w, TAPS, 0, FR, bias=bias)
+    steps, S = _f_steps(), 4
+    parts = [_f_acc(a, FH, w, steps[len(steps) * p // S:len(steps) * (p + 1) // S]) for p in range(S)]
+
+    def finish(slots):
+        acc = torch.zeros_like(parts[0])
+        for t in slots:
+            acc += t
+        return (acc + bias).half()
+    assert M.c_f(finish(parts), ref, mag, "f16") <= M.C_TOL / 4
+    c = M.c_f(finish(parts[:-1]), ref, mag, "f16")
+    print("form F planted finisher_drops_a_partial: c = %.3g" % c)
+    assert c > 20 * M.C_TOL
 
 
 # ------------------------------------------------------------------------------------------------------
