@@ -3,10 +3,11 @@
 // Both kernels are persistent (at most one CTA per SM, static round-robin tile schedule) and warp
 // specialised by warpgroup -- warpgroup 0: TMA producer (one thread issues, the others give their
 // registers back with setmaxnreg), warpgroups 1 and 2: consumers, each owning 64 of the tile's 128 M rows
-// with its fp32 accumulator in registers (wgmma m64nNk16, N = the tile's width).  A 4-stage shared-memory
-// ring (full / empty mbarriers) keeps the producer ahead of the consumers, so the loads of tile i+1 overlap
-// the epilogue of tile i.  Form F stages whole 16-bit output tiles in shared memory and writes them with TMA
-// stores that drain during the next tile's MMAs (f_epilogue_tma); the other epilogues store from the fragment.
+// with its fp32 accumulator in registers (wgmma m64nNk16, N = the tile's width).  A shared-memory ring
+// (full / empty mbarriers, 4 stages; form F sizes them to the tile width, see FSmem) keeps the producer ahead of the
+// consumers, so the loads of tile i+1 overlap the epilogue of tile i.  Form F stages whole 16-bit output tiles in
+// shared memory and writes them with TMA stores that drain during the next tile's MMAs (f_epilogue_tma); the
+// other epilogues store from the fragment.
 //
 // Every operand tile is a TMA box of 64 channels (128 B) x rows, 128B-swizzled, so the same
 // shared-memory bytes serve as
@@ -91,6 +92,9 @@ __device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, uint32_t sr
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // every bulk store this thread issued has finished READING shared memory (the global writes may still be in flight)
 __device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// ... all but the N most recently committed bulk groups of this thread
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
 // this thread's generic-proxy shared-memory writes become visible to the async proxy (TMA)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
@@ -228,14 +232,31 @@ constexpr int A_STAGE_BYTES = 128 * 128;   // 128 rows x 128 B
 constexpr int B_STAGE_BYTES = 256 * 128;   // up to 256 rows x 128 B
 constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
 constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/ + 2048 /*column statistics*/;
-// form F: the ring, then the output staging area (two 16 KB slots, each one 128-row x 64-column 16-bit chunk of a
-// tile, 1024 B aligned for the 128B swizzle; the BatchNorm column statistics alias it, their launches store
-// directly), then the barriers
+constexpr int SMEM_OPTIN_LIMIT = 232448;   // sm_90 per-block opt-in maximum
+// Form F, per tile width TN: a ring of stages sized to the tile (16 KB of A + TN x 128 B of weights), then the output
+// staging area of 16 KB chunks (each one 128-row x 64-column 16-bit chunk of a tile, 1024 B aligned for the 128B
+// swizzle; the BatchNorm column statistics alias it, their launches store from the fragment), then the barriers.
+//   TN  64: 4 x 24 KB ring, two 32 KB buffers used by alternate tiles, each a whole tile with out2: the single-tap
+//           launches are store-bound, so a tile's staging must not wait for the previous tile's stores
+//   TN 128: 4 x 32 KB ring, one 64 KB buffer: a whole tile with out2
+//   TN 256: 4 x 48 KB ring, one 32 KB buffer: the tile leaves in rounds of two chunks.  Nothing larger fits next to
+//           four stages, and a 3-stage ring lengthens the main loop of the 256-wide layers by more than whole-tile
+//           staging saves
 constexpr int OUT_CHUNK_BYTES = 128 * 128;
-constexpr int OUT_STAGE_OFF = STAGES * STAGE_BYTES;
-constexpr int F_CTL_OFF = OUT_STAGE_OFF + 2 * OUT_CHUNK_BYTES;
-constexpr int F_SMEM_BYTES = F_CTL_OFF + 256 /*barriers*/ + 1024 /*align*/;
-static_assert(F_SMEM_BYTES <= 232448, "form-F shared memory exceeds the sm_90 opt-in limit");
+template <int TN>
+struct FSmem {
+  static constexpr int RING = 4;
+  static constexpr int STAGE_BYTES = A_STAGE_BYTES + TN * 128;
+  static constexpr int BUFS = TN == 64 ? 2 : 1;                   // staging buffers, used by alternate tiles
+  static constexpr int BUF_BYTES = (TN == 256 ? 2 : 4) * OUT_CHUNK_BYTES / BUFS;
+  static constexpr int STG_OFF = RING * STAGE_BYTES;
+  static constexpr int CTL_OFF = STG_OFF + BUFS * BUF_BYTES;
+  static constexpr int BYTES = CTL_OFF + 256 /*barriers*/ + 1024 /*align*/;
+  static_assert(RING <= STAGES && STAGE_BYTES % 1024 == 0 && BUFS * BUF_BYTES >= 2048, "form-F shared memory");
+};
+static_assert(FSmem<64>::BYTES <= SMEM_OPTIN_LIMIT, "form-F TN 64 shared memory exceeds the sm_90 opt-in limit");
+static_assert(FSmem<128>::BYTES <= SMEM_OPTIN_LIMIT, "form-F TN 128 shared memory exceeds the sm_90 opt-in limit");
+static_assert(FSmem<256>::BYTES <= SMEM_OPTIN_LIMIT, "form-F TN 256 shared memory exceeds the sm_90 opt-in limit");
 constexpr int NUM_THREADS = 384;           // producer warpgroup + two consumer warpgroups
 constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 
@@ -480,25 +501,39 @@ __device__ __forceinline__ void f_epilogue(const FTcParams& p, float (&acc)[TN /
 }
 
 // Epilogue of a whole tile with a 16-bit `out` (every forward and data-gradient launch but fc.0 and BatchNorm-stat
-// launches), all 256 consumer threads together.  The tile leaves in 64-column chunks: the consumers write a chunk
-// into a 16 KB staging slot (rows in fragment order tb * TR + tr = the box's row order, 128B-swizzled so that the
-// 8 rows of one warp store hit different banks) and one thread writes the slot with a TMA tensor store whose box
-// {64, TR, TB} is clipped at the launch's columns, rows and batch elements.  Two slots: two chunks of `out` per
-// round, or a chunk of `out` and the same chunk of `out2`.  The stores of the last round drain while the consumers
-// run the next tile's MMAs; a slot is rewritten only after the issuing thread has seen its bulk group finish reading
-// (next round or next tile).  Per element the arithmetic is f_store2's: fp32 accumulator + bias, PReLU from fp32,
-// one rounding.  The reflect-halo mirror rows of out2 (rows reversed: no box expresses them) are copied from the
-// staged chunk with 16-byte stores.
-template <int TN>
-__device__ __forceinline__ void f_epilogue_tma(const FTcParams& p, const float (&acc)[TN / 2], int mt, int n0,
-                                               int ctid, uint32_t stg, const CUtensorMap* tmO,
-                                               const CUtensorMap* tmO2) {
+// launches), all 256 consumer threads together.  The consumers write the tile into a staging buffer `buf` in
+// 64-column chunks of 16 KB (rows in fragment order tb * TR + tr = the box's row order, 128B-swizzled so that the 8
+// rows of one warp store hit different banks), then one thread issues a TMA tensor store per chunk, box {64, TR, TB}
+// clipped at the launch's columns, rows and batch elements, and commits them as one bulk group.  The consumers go
+// straight back to the MMAs while the stores drain; a buffer is rewritten only after the issuing thread has seen the
+// bulk group that last read it finish reading (FSmem: with two buffers that is the group before the last one).  At
+// TN 256 the buffer holds two chunks, so the tile leaves in rounds with such a wait between them (two chunks of
+// `out`, or a chunk of `out` and the same chunk of `out2`).
+// Per element the arithmetic is f_store2's: fp32 accumulator + bias, PReLU from fp32, one rounding.  The
+// reflect-halo mirror rows of out2 (rows reversed: no box expresses them) are copied from the staged chunks with
+// 16-byte stores.
+// The body is fully unrolled over the tile's TN / 4 column pairs per thread, so everything that is uniform over the
+// tile stays out of it: the output format F16 and MODE (0: out; 1: PReLU applied to out; 2: out and the PReLU
+// output out2) are template parameters chosen once per tile, and the bias / slope column of each 64-column chunk is
+// reduced modulo bias_mod / slope_mod once (both are multiples of 64, as is n0: a chunk never wraps), so a pair's
+// parameters are two loads at fixed offsets.
+template <bool F16>
+__device__ __forceinline__ uint32_t pack2_t(float x, float y) {
+  if constexpr (F16) return pack_half2_sat(x, y);
+  __nv_bfloat162 h = __floats2bfloat162_rn(x, y);
+  return *reinterpret_cast<uint32_t*>(&h);
+}
+
+template <int TN, bool F16, int MODE>
+__device__ __forceinline__ void f_epilogue_tma_body(const FTcParams& p, const float (&acc)[TN / 2], int mt, int n0,
+                                                    int ctid, uint32_t buf, const CUtensorMap* tmO,
+                                                    const CUtensorMap* tmO2) {
+  constexpr bool two = MODE == 2;
+  constexpr bool act_in_place = MODE == 1;
   const int lane = ctid & 31, cw = ctid >> 5;
   const int mtb = p.m_tiles_per_b == 1 ? mt : mt / p.m_tiles_per_b;
   const int b0 = mtb * p.TB;
   const int m0 = p.m_lo + (mt - mtb * p.m_tiles_per_b) * p.TR;
-  const bool two = p.out2 != nullptr;
-  const bool act_in_place = p.slope != nullptr && !two;
   const bool add_bias = p.bias != nullptr;
   // this thread's 4-byte word of row cw * 16 + lane / 4 (+ 8 for h = 1, 1024 B further) in a staged chunk; the
   // row's 16-byte column block jj sits at block jj ^ (row & 7) = jj ^ (lane / 4)
@@ -508,55 +543,56 @@ __device__ __forceinline__ void f_epilogue_tma(const FTcParams& p, const float (
   const bool mirror_tile = two && halo2 > 0 &&
                            ((m0 <= halo2 && m0 + p.TR > 1) || (m0 + p.TR > p.out_rows - 1 - halo2 && m0 <= p.out_rows - 2));
   constexpr int NQ = TN / 64;
+  // A round stages as many 64-column chunks as the buffer holds (CH slots; with out2 each chunk of out takes two
+  // slots, out's and out2's), issues their stores and commits them as one bulk group.
+  constexpr int CH = FSmem<TN>::BUF_BYTES / OUT_CHUNK_BYTES;
+  constexpr int QPR = two ? CH / 2 : CH;          // chunks per round
+  const int c_rel = n0 - p.n_lo, m_rel = m0 - p.m_lo;
 #pragma unroll
   for (int q = 0; q < NQ; ++q) {
-    const bool round_start = two || (q & 1) == 0;
-    const bool round_end = two || (q & 1) == 1 || q == NQ - 1;
-    const uint32_t slot = stg + (two ? 0u : (uint32_t)(q & 1) * OUT_CHUNK_BYTES);
-    if (round_start) {
-      if (ctid == 0) bulk_wait_read_all();        // the slots' previous stores have read them ...
-      consumer_bar_sync();                        // ... before anyone writes them again
+    const int qi = q % QPR;                       // position in the round
+    const uint32_t slot = buf + (uint32_t)(two ? 2 * qi : qi) * OUT_CHUNK_BYTES;
+    if (qi == 0) {
+      if (ctid == 0) {                            // the stores that last read this buffer are done reading ...
+        if (q == 0) bulk_wait_read<FSmem<TN>::BUFS - 1>();
+        else bulk_wait_read<0>();
+      }
+      consumer_bar_sync();                        // ... before anyone writes it again
     }
+    // this thread's first column of the chunk: n0 + 64 q + 2 (lane % 4); column pair jj is 8 jj further
+    const int cq0 = n0 + 64 * q;
+    const float* bq = p.bias + f_mod(cq0, p.bias_mod, p.bias_mask) + 2 * (lane & 3);
+    const float* sq = p.slope + (MODE != 0 ? f_mod(cq0, p.slope_mod, p.slope_mask) + 2 * (lane & 3) : 0);
 #pragma unroll
     for (int jj = 0; jj < 8; ++jj) {
       const int j = 8 * q + jj;
-      const int c = 8 * j + 2 * (lane & 3);
       float bx = 0.f, by = 0.f;
-      if (add_bias) {    // bias_mod is a multiple of 64: no wrap inside the pair
-        const float* bp = p.bias + f_mod(n0 + c, p.bias_mod, p.bias_mask);
-        bx = __ldg(bp); by = __ldg(bp + 1);
-      }
+      if (add_bias) { bx = __ldg(bq + 8 * jj); by = __ldg(bq + 8 * jj + 1); }
       float s0 = 0.f, s1 = 0.f;
-      if (p.slope != nullptr) {
-        const float* sp = p.slope + f_mod(n0 + c, p.slope_mod, p.slope_mask);
-        s0 = __ldg(sp); s1 = __ldg(sp + 1);
-      }
+      if constexpr (MODE != 0) { s0 = __ldg(sq + 8 * jj); s1 = __ldg(sq + 8 * jj + 1); }
       const uint32_t col_off = (uint32_t)((jj ^ sw) << 4);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         float x = acc[4 * j + 2 * h] + bx, y = acc[4 * j + 2 * h + 1] + by;
-        if (act_in_place) {
+        if constexpr (act_in_place) {
           x = x > 0.f ? x : s0 * x;
           y = y > 0.f ? y : s1 * y;
         }
         const uint32_t off = row_off + (uint32_t)h * 1024u + col_off;
-        st_shared_u32(slot + off, pack2(x, y, p.out_dtype));
-        if (two) st_shared_u32(slot + OUT_CHUNK_BYTES + off, pack2(x > 0.f ? x : s0 * x, y > 0.f ? y : s1 * y, p.out_dtype));
+        st_shared_u32(slot + off, pack2_t<F16>(x, y));
+        if constexpr (two) st_shared_u32(slot + OUT_CHUNK_BYTES + off, pack2_t<F16>(x > 0.f ? x : s0 * x, y > 0.f ? y : s1 * y));
       }
     }
-    if (!round_end) continue;
+    if (qi != QPR - 1 && q != NQ - 1) continue;
     fence_proxy_async_smem();
     consumer_bar_sync();
     if (ctid == 0) {
-      const int c_rel = n0 - p.n_lo + 64 * q, m_rel = m0 - p.m_lo;
-      if (two) {
-        tma_store_3d(tmO, slot, c_rel, m_rel, b0);
-        tma_store_3d(tmO2, slot + OUT_CHUNK_BYTES, c_rel, m_rel, b0);
-      } else if (q & 1) {
-        tma_store_3d(tmO, stg, c_rel - 64, m_rel, b0);
-        tma_store_3d(tmO, stg + OUT_CHUNK_BYTES, c_rel, m_rel, b0);
-      } else {
-        tma_store_3d(tmO, stg, c_rel, m_rel, b0);
+#pragma unroll
+      for (int k = 0; k <= qi; ++k) {
+        const uint32_t src = buf + (uint32_t)(two ? 2 * k : k) * OUT_CHUNK_BYTES;
+        const int cq = c_rel + 64 * (q - qi + k);
+        tma_store_3d(tmO, src, cq, m_rel, b0);
+        if constexpr (two) tma_store_3d(tmO2, src + OUT_CHUNK_BYTES, cq, m_rel, b0);
       }
       bulk_commit();
     }
@@ -564,8 +600,9 @@ __device__ __forceinline__ void f_epilogue_tma(const FTcParams& p, const float (
       // out2 rows m in [1, halo] also land on row -m, rows m in [out_rows-1-halo, out_rows-2] on 2(out_rows-1)-m
       const int rows = p.TR * p.TB;
       const int out2_buf_rows = p.out_rows + 2 * halo2;
-      for (int idx = ctid; idx < rows * 8; idx += 256) {
-        const int r = idx >> 3, k = idx & 7;
+      for (int idx = ctid; idx < rows * 8 * (qi + 1); idx += 256) {
+        const int k = idx / (rows * 8), rk = idx - k * rows * 8;
+        const int r = rk >> 3, kb = rk & 7;
         const int tb = r / p.TR, tr = r - tb * p.TR;
         const int b = b0 + tb, m = m0 + tr;
         if (b >= p.batch || m >= p.m_hi) continue;
@@ -573,11 +610,29 @@ __device__ __forceinline__ void f_epilogue_tma(const FTcParams& p, const float (
         if (m >= 1 && m <= halo2) mm = -m;
         else if (m >= p.out_rows - 1 - halo2 && m <= p.out_rows - 2) mm = 2 * (p.out_rows - 1) - m;
         else continue;
-        const uint4 v = ld_shared_v4(slot + OUT_CHUNK_BYTES + (uint32_t)r * 128u + (uint32_t)((k ^ (r & 7)) << 4));
-        const int64_t o = ((int64_t)b * out2_buf_rows + halo2 + mm) * p.out_ld + p.out_col0 + (n0 - p.n_lo) + 64 * q + 8 * k;
+        const uint32_t src = buf + (uint32_t)(2 * k + 1) * OUT_CHUNK_BYTES;
+        const uint4 v = ld_shared_v4(src + (uint32_t)r * 128u + (uint32_t)((kb ^ (r & 7)) << 4));
+        const int64_t o = ((int64_t)b * out2_buf_rows + halo2 + mm) * p.out_ld + p.out_col0 + c_rel +
+                          64 * (q - qi + k) + 8 * kb;
         *reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.out2) + o) = v;
       }
     }
+  }
+}
+
+template <int TN>
+__device__ __forceinline__ void f_epilogue_tma(const FTcParams& p, const float (&acc)[TN / 2], int mt, int n0,
+                                               int ctid, uint32_t buf, const CUtensorMap* tmO,
+                                               const CUtensorMap* tmO2) {
+  const int mode = p.out2 != nullptr ? 2 : (p.slope != nullptr ? 1 : 0);
+  if (p.out_dtype == SG_F16) {
+    if (mode == 2) f_epilogue_tma_body<TN, true, 2>(p, acc, mt, n0, ctid, buf, tmO, tmO2);
+    else if (mode == 1) f_epilogue_tma_body<TN, true, 1>(p, acc, mt, n0, ctid, buf, tmO, tmO2);
+    else f_epilogue_tma_body<TN, true, 0>(p, acc, mt, n0, ctid, buf, tmO, tmO2);
+  } else {
+    if (mode == 2) f_epilogue_tma_body<TN, false, 2>(p, acc, mt, n0, ctid, buf, tmO, tmO2);
+    else if (mode == 1) f_epilogue_tma_body<TN, false, 1>(p, acc, mt, n0, ctid, buf, tmO, tmO2);
+    else f_epilogue_tma_body<TN, false, 0>(p, acc, mt, n0, ctid, buf, tmO, tmO2);
   }
 }
 
@@ -595,8 +650,9 @@ tapgemm_f_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ C
              const __grid_constant__ CUtensorMap tmO2, const FTcParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  SharedCtl* ctl = reinterpret_cast<SharedCtl*>(smem + F_CTL_OFF);
-  float* colstat = reinterpret_cast<float*>(smem + OUT_STAGE_OFF);      // [2][256], aliases the output staging
+  using L = FSmem<TN>;
+  SharedCtl* ctl = reinterpret_cast<SharedCtl*>(smem + L::CTL_OFF);
+  float* colstat = reinterpret_cast<float*>(smem + L::STG_OFF);      // [2][256], aliases the output staging
   const int wg = threadIdx.x >> 7;
 
   if (threadIdx.x == 0) {
@@ -605,7 +661,7 @@ tapgemm_f_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ C
       prefetch_tmap(&tmO);
       if (p.out2 != nullptr) prefetch_tmap(&tmO2);
     }
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&ctl->full[s], 1); mbar_init(&ctl->empty[s], 2); }
+    for (int s = 0; s < L::RING; ++s) { mbar_init(&ctl->full[s], 1); mbar_init(&ctl->empty[s], 2); }
     fence_barrier_init();
   }
   if (p.stats != nullptr)
@@ -661,12 +717,12 @@ tapgemm_f_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ C
               next_sel += p.ksplit;
             }
             mbar_wait(&ctl->empty[stage], phase ^ 1);
-            uint8_t* sa = smem + stage * STAGE_BYTES;
+            uint8_t* sa = smem + stage * L::STAGE_BYTES;
             mbar_expect_tx(&ctl->full[stage], a_bytes + b_bytes);
             if (k0 < p.a0_c) tma_load_3d(sa, &tmA0, &ctl->full[stage], k0, m0 + d + p.a_halo, b0);
             else tma_load_3d(sa, &tmA1, &ctl->full[stage], k0 - p.a0_c, m0 + d + p.a_halo, b0);
             tma_load_2d(sa + A_STAGE_BYTES, &tmW, &ctl->full[stage], k0, (ti - p.w_tap0) * p.nc + n0);
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            if (++stage == L::RING) { stage = 0; phase ^= 1; }
           }
           step += nk;
         }
@@ -700,6 +756,7 @@ tapgemm_f_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ C
   unsigned long long* tl = g_tc_timeline + (blockIdx.x < TL_CTAS ? blockIdx.x : 0) * TL_SLOTS;
   if (tl_on) { for (int i = 0; i < TL_SLOTS; ++i) tl[i] = 0; tl[tl_i++] = gtime_ns(); }
 
+  int staged = 0;                                  // tiles this CTA has staged (selects the staging buffer)
   float acc[TN / 2];
   while (it.next(p, pc)) {
     const int ks = p.ksplit == 1 ? 0 : pc.rest % p.ksplit;
@@ -718,21 +775,23 @@ tapgemm_f_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ C
     int prev = 0;
     for (int i = 0; i < nsteps; ++i) {
       mbar_wait(&ctl->full[stage], phase);
-      const uint32_t sa = smem0 + (uint32_t)stage * STAGE_BYTES;
+      const uint32_t sa = smem0 + (uint32_t)stage * L::STAGE_BYTES;
       mma_k64<TN, 0, 0, BF16>(acc, make_smem_desc(sa + (uint32_t)cwg * 8192u, 16, 1024),
                         make_smem_desc(sa + A_STAGE_BYTES, 16, 1024), 2, 2, i == 0);
       wgmma_wait<1>();                               // the MMAs of step i-1 have retired: free their stage
       if (i > 0 && wg_leader) mbar_arrive(&ctl->empty[prev]);
       prev = stage;
-      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      if (++stage == L::RING) { stage = 0; phase ^= 1; }
     }
     wgmma_wait<0>();
     if (nsteps > 0 && wg_leader) mbar_arrive(&ctl->empty[prev]);
     if (tl_on && tl_i < TL_SLOTS - 1) tl[tl_i++] = gtime_ns();
 
     if (!partial) {
-      if (p.tma_out) f_epilogue_tma<TN>(p, acc, pc.mt, n0, ctid, smem0 + OUT_STAGE_OFF, &tmO, &tmO2);
-      else f_epilogue<TN>(p, acc, pc.mt, n0, ks, ctid, colstat);
+      if (p.tma_out) {
+        const uint32_t buf = smem0 + L::STG_OFF + (uint32_t)(staged++ % L::BUFS) * L::BUF_BYTES;
+        f_epilogue_tma<TN>(p, acc, pc.mt, n0, ctid, buf, &tmO, &tmO2);
+      } else f_epilogue<TN>(p, acc, pc.mt, n0, ks, ctid, colstat);
       if (tl_on && tl_i < TL_SLOTS - 1) tl[tl_i++] = gtime_ns();
       continue;
     }
@@ -1115,13 +1174,14 @@ int tapgemm_f_tc_launch(const sg_tapgemm_f* q, cudaStream_t st) {
   }
   const bool bf = q->a_dtype == SG_BF16;
   void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, FTcParams);
-  if (p.TN == 256) kern = bf ? tapgemm_f_tc<256, true> : tapgemm_f_tc<256, false>;
-  else if (p.TN == 128) kern = bf ? tapgemm_f_tc<128, true> : tapgemm_f_tc<128, false>;
-  else kern = bf ? tapgemm_f_tc<64, true> : tapgemm_f_tc<64, false>;
-  SG_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, F_SMEM_BYTES));
+  int smem_bytes;
+  if (p.TN == 256) { kern = bf ? tapgemm_f_tc<256, true> : tapgemm_f_tc<256, false>; smem_bytes = FSmem<256>::BYTES; }
+  else if (p.TN == 128) { kern = bf ? tapgemm_f_tc<128, true> : tapgemm_f_tc<128, false>; smem_bytes = FSmem<128>::BYTES; }
+  else { kern = bf ? tapgemm_f_tc<64, true> : tapgemm_f_tc<64, false>; smem_bytes = FSmem<64>::BYTES; }
+  SG_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
   void* args[] = {&tmA0, &tmA1, &tmW, &tmO, &tmO2, &p};
   SG_CHECK_CUDA(cudaLaunchKernel(reinterpret_cast<const void*>(kern), dim3(nctas), dim3(NUM_THREADS), args,
-                                 (size_t)F_SMEM_BYTES, st));
+                                 (size_t)smem_bytes, st));
   return SG_OK;
 }
 
