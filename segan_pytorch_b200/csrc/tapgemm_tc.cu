@@ -273,8 +273,10 @@ struct FTcParams {
   int m_lo, m_hi, n_lo;
   const float* bias; int bias_mod;
   int batch, ksplit;
-  int TR, TB, TN;            // M tile = TB batches x TR rows (<= 128), N tile
-  int m_tiles_per_b, b_tiles, n_tiles;
+  int TR, TB, TN;            // segment 0's M tile = TB batches x TR rows (<= 128), N tile
+  int m_tiles_per_b, n_tiles;
+  int m_tiles0, m_tiles;     // M tiles of segment 0 (m_tiles_per_b x its batch tiles), of both segments
+  int m_lo1, TR1, TB1;       // segment 1 (rows [m_lo1, m_hi), TR1 < 128 of them, TB1 batches per tile), TR1 = 0: none
   int dbg;                   // SEGAN_B200_DEBUG (bit 20: phase timeline)
   double* stats;             // fused BatchNorm statistics [SG_STAT_SLICES][2][nc], or nullptr
   int sk_dp_tiles;           // tiles [0, sk_dp_tiles) are tile-strided; each of the rest is split along K over
@@ -287,6 +289,9 @@ struct FTcParams {
   int bias_mask, slope_mask; // mod - 1 when the modulus is a power of two (the channel counts are), else -1
   int tma_out;               // whole tiles leave through shared memory and TMA stores (16-bit out, no BatchNorm stats)
 };
+
+// tapgemm_f_tc's parameters: eight tensor maps and FTcParams, inside the classic 4 KB kernel-parameter space
+static_assert(8 * sizeof(CUtensorMap) + sizeof(FTcParams) <= 4096, "tapgemm_f_tc parameter block exceeds 4 KB");
 
 struct SharedCtl {
   uint64_t full[STAGES];
@@ -381,6 +386,30 @@ struct PieceIter {
   }
 };
 
+// Rows of M tile mt.  A launch's rows [m_lo, m_hi) are one or two segments, each packed into M tiles of TB batch
+// elements x TR rows (tapgemm_f_tc_launch).  Segment 0's tiles come first (row tile fastest, then batch tile);
+// segment 1, the last TR1 rows of every batch element, follows with one tile per TB1 batch elements.  The tile covers
+// batch elements [b0, b0 + TB) x rows [m0, m0 + TR); m_rel is m0 relative to the first row of its segment's store map.
+struct FTile {
+  int b0, m0, m_rel, TR, TB, seg;
+};
+__device__ __forceinline__ FTile f_tile(const FTcParams& p, int mt) {
+  FTile t;
+  if (mt < p.m_tiles0) {
+    const int mtb = p.m_tiles_per_b == 1 ? mt : mt / p.m_tiles_per_b;
+    t.b0 = mtb * p.TB;
+    t.m_rel = (mt - mtb * p.m_tiles_per_b) * p.TR;
+    t.m0 = p.m_lo + t.m_rel;
+    t.TR = p.TR; t.TB = p.TB; t.seg = 0;
+  } else {
+    t.b0 = (mt - p.m_tiles0) * p.TB1;
+    t.m_rel = 0;
+    t.m0 = p.m_lo1;
+    t.TR = p.TR1; t.TB = p.TB1; t.seg = 1;
+  }
+  return t;
+}
+
 __device__ __forceinline__ int f_mod(int x, int mod, int mask) { return mask >= 0 ? (x & mask) : (x % mod); }
 
 __device__ __forceinline__ uint32_t pack2(float x, float y, int dtype) {
@@ -430,23 +459,20 @@ __device__ __forceinline__ float round_as_stored(float x, int dtype) {
 // statistics into shared memory).  Fragment layout of m64nN: consumer warp cw (0..7) owns tile rows 16 cw + lane/4
 // and 16 cw + 8 + lane/4; register 4j + 2h + e holds column 8j + 2(lane%4) + e of the h-th of those rows.
 template <int TN>
-__device__ __forceinline__ void f_epilogue(const FTcParams& p, float (&acc)[TN / 2], int mt, int n0, int ks, int ctid,
-                                           float* colstat) {
+__device__ __forceinline__ void f_epilogue(const FTcParams& p, float (&acc)[TN / 2], const FTile& t, int n0, int ks,
+                                           int ctid, float* colstat) {
   const int lane = ctid & 31, cw = ctid >> 5;
   const int out_buf_rows = p.out_rows + 2 * p.out_halo;
   const int out2_buf_rows = p.out_rows + 2 * p.out2_halo;
-  const int mtb = p.m_tiles_per_b == 1 ? mt : mt / p.m_tiles_per_b;
-  const int b0 = mtb * p.TB;
-  const int m0 = p.m_lo + (mt - mtb * p.m_tiles_per_b) * p.TR;
   const int col0 = n0 - p.n_lo + p.out_col0 + 2 * (lane & 3);
   int64_t obase[2], o2base[2], o2mirror[2];
   bool valid[2];
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int r = cw * 16 + (lane >> 2) + 8 * h;
-    const int tb = r / p.TR, tr = r - tb * p.TR;
-    const int b = b0 + tb, m = m0 + tr;
-    valid[h] = (tb < p.TB) && (b < p.batch) && (m < p.m_hi);
+    const int tb = r / t.TR, tr = r - tb * t.TR;
+    const int b = t.b0 + tb, m = t.m0 + tr;
+    valid[h] = (tb < t.TB) && (b < p.batch) && (m < p.m_hi);
     obase[h] = ((int64_t)b * out_buf_rows + (m + p.out_halo)) * p.out_ld + col0;
     o2base[h] = 0; o2mirror[h] = -1;
     if (p.out2 != nullptr) {
@@ -525,15 +551,13 @@ __device__ __forceinline__ uint32_t pack2_t(float x, float y) {
 }
 
 template <int TN, bool F16, int MODE>
-__device__ __forceinline__ void f_epilogue_tma_body(const FTcParams& p, const float (&acc)[TN / 2], int mt, int n0,
-                                                    int ctid, uint32_t buf, const CUtensorMap* tmO,
+__device__ __forceinline__ void f_epilogue_tma_body(const FTcParams& p, const float (&acc)[TN / 2], const FTile& t,
+                                                    int n0, int ctid, uint32_t buf, const CUtensorMap* tmO,
                                                     const CUtensorMap* tmO2) {
   constexpr bool two = MODE == 2;
   constexpr bool act_in_place = MODE == 1;
   const int lane = ctid & 31, cw = ctid >> 5;
-  const int mtb = p.m_tiles_per_b == 1 ? mt : mt / p.m_tiles_per_b;
-  const int b0 = mtb * p.TB;
-  const int m0 = p.m_lo + (mt - mtb * p.m_tiles_per_b) * p.TR;
+  const int b0 = t.b0, m0 = t.m0;
   const bool add_bias = p.bias != nullptr;
   // this thread's 4-byte word of row cw * 16 + lane / 4 (+ 8 for h = 1, 1024 B further) in a staged chunk; the
   // row's 16-byte column block jj sits at block jj ^ (row & 7) = jj ^ (lane / 4)
@@ -541,13 +565,13 @@ __device__ __forceinline__ void f_epilogue_tma_body(const FTcParams& p, const fl
   const int sw = lane >> 2;
   const int halo2 = p.out2_halo;
   const bool mirror_tile = two && halo2 > 0 &&
-                           ((m0 <= halo2 && m0 + p.TR > 1) || (m0 + p.TR > p.out_rows - 1 - halo2 && m0 <= p.out_rows - 2));
+                           ((m0 <= halo2 && m0 + t.TR > 1) || (m0 + t.TR > p.out_rows - 1 - halo2 && m0 <= p.out_rows - 2));
   constexpr int NQ = TN / 64;
   // A round stages as many 64-column chunks as the buffer holds (CH slots; with out2 each chunk of out takes two
   // slots, out's and out2's), issues their stores and commits them as one bulk group.
   constexpr int CH = FSmem<TN>::BUF_BYTES / OUT_CHUNK_BYTES;
   constexpr int QPR = two ? CH / 2 : CH;          // chunks per round
-  const int c_rel = n0 - p.n_lo, m_rel = m0 - p.m_lo;
+  const int c_rel = n0 - p.n_lo, m_rel = t.m_rel;
 #pragma unroll
   for (int q = 0; q < NQ; ++q) {
     const int qi = q % QPR;                       // position in the round
@@ -598,12 +622,12 @@ __device__ __forceinline__ void f_epilogue_tma_body(const FTcParams& p, const fl
     }
     if (mirror_tile) {
       // out2 rows m in [1, halo] also land on row -m, rows m in [out_rows-1-halo, out_rows-2] on 2(out_rows-1)-m
-      const int rows = p.TR * p.TB;
+      const int rows = t.TR * t.TB;
       const int out2_buf_rows = p.out_rows + 2 * halo2;
       for (int idx = ctid; idx < rows * 8 * (qi + 1); idx += 256) {
         const int k = idx / (rows * 8), rk = idx - k * rows * 8;
         const int r = rk >> 3, kb = rk & 7;
-        const int tb = r / p.TR, tr = r - tb * p.TR;
+        const int tb = r / t.TR, tr = r - tb * t.TR;
         const int b = b0 + tb, m = m0 + tr;
         if (b >= p.batch || m >= p.m_hi) continue;
         int mm;
@@ -621,18 +645,18 @@ __device__ __forceinline__ void f_epilogue_tma_body(const FTcParams& p, const fl
 }
 
 template <int TN>
-__device__ __forceinline__ void f_epilogue_tma(const FTcParams& p, const float (&acc)[TN / 2], int mt, int n0,
+__device__ __forceinline__ void f_epilogue_tma(const FTcParams& p, const float (&acc)[TN / 2], const FTile& t, int n0,
                                                int ctid, uint32_t buf, const CUtensorMap* tmO,
                                                const CUtensorMap* tmO2) {
   const int mode = p.out2 != nullptr ? 2 : (p.slope != nullptr ? 1 : 0);
   if (p.out_dtype == SG_F16) {
-    if (mode == 2) f_epilogue_tma_body<TN, true, 2>(p, acc, mt, n0, ctid, buf, tmO, tmO2);
-    else if (mode == 1) f_epilogue_tma_body<TN, true, 1>(p, acc, mt, n0, ctid, buf, tmO, tmO2);
-    else f_epilogue_tma_body<TN, true, 0>(p, acc, mt, n0, ctid, buf, tmO, tmO2);
+    if (mode == 2) f_epilogue_tma_body<TN, true, 2>(p, acc, t, n0, ctid, buf, tmO, tmO2);
+    else if (mode == 1) f_epilogue_tma_body<TN, true, 1>(p, acc, t, n0, ctid, buf, tmO, tmO2);
+    else f_epilogue_tma_body<TN, true, 0>(p, acc, t, n0, ctid, buf, tmO, tmO2);
   } else {
-    if (mode == 2) f_epilogue_tma_body<TN, false, 2>(p, acc, mt, n0, ctid, buf, tmO, tmO2);
-    else if (mode == 1) f_epilogue_tma_body<TN, false, 1>(p, acc, mt, n0, ctid, buf, tmO, tmO2);
-    else f_epilogue_tma_body<TN, false, 0>(p, acc, mt, n0, ctid, buf, tmO, tmO2);
+    if (mode == 2) f_epilogue_tma_body<TN, false, 2>(p, acc, t, n0, ctid, buf, tmO, tmO2);
+    else if (mode == 1) f_epilogue_tma_body<TN, false, 1>(p, acc, t, n0, ctid, buf, tmO, tmO2);
+    else f_epilogue_tma_body<TN, false, 0>(p, acc, t, n0, ctid, buf, tmO, tmO2);
   }
 }
 
@@ -642,12 +666,16 @@ __device__ __forceinline__ void f_epilogue_tma(const FTcParams& p, const float (
 //   K = 64-channel blocks.  Optional: interleaved K split into fp32 (ksplit > 1, vector red), stream-K tail,
 //   fused BatchNorm statistics, fused PReLU / second output.
 // ------------------------------------------------------------------------------------------
-// BF16: operand format (bf16 / fp16), a template parameter so that each wgmma has one fixed form
+// BF16: operand format (bf16 / fp16), a template parameter so that each wgmma has one fixed form.
+// tmA0 / tmA1 / tmO: the A source and `out` maps of row segment 0 (boxes {64, TR, TB}); tmA0s1 / tmA1s1 / tmOs1:
+// those of segment 1 (boxes {64, TR1, TB1}; copies of segment 0's when TR1 = 0).  out2 launches never split.
 template <int TN, bool BF16>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 tapgemm_f_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
              const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmO,
-             const __grid_constant__ CUtensorMap tmO2, const FTcParams p) {
+             const __grid_constant__ CUtensorMap tmO2, const __grid_constant__ CUtensorMap tmA0s1,
+             const __grid_constant__ CUtensorMap tmA1s1, const __grid_constant__ CUtensorMap tmOs1,
+             const FTcParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   using L = FSmem<TN>;
@@ -661,6 +689,10 @@ tapgemm_f_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ C
       prefetch_tmap(&tmO);
       if (p.out2 != nullptr) prefetch_tmap(&tmO2);
     }
+    if (p.TR1 > 0) {
+      prefetch_tmap(&tmA0s1); prefetch_tmap(&tmA1s1);
+      if (p.tma_out) prefetch_tmap(&tmOs1);
+    }
     for (int s = 0; s < L::RING; ++s) { mbar_init(&ctl->full[s], 1); mbar_init(&ctl->empty[s], 2); }
     fence_barrier_init();
   }
@@ -668,12 +700,10 @@ tapgemm_f_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ C
     for (int c = threadIdx.x; c < 512; c += NUM_THREADS) colstat[c] = 0.f;
   __syncthreads();
 
-  const int m_tiles = p.m_tiles_per_b * p.b_tiles;
-  const int total_tiles = m_tiles * p.n_tiles * p.ksplit;
-  const uint32_t a_bytes = (uint32_t)p.TR * p.TB * 128u;
+  const int total_tiles = p.m_tiles * p.n_tiles * p.ksplit;
   const uint32_t b_bytes = (uint32_t)TN * 128u;
   PieceIter it;
-  it.init(p, m_tiles, total_tiles, blockIdx.x, gridDim.x);
+  it.init(p, p.m_tiles, total_tiles, blockIdx.x, gridDim.x);
   Piece pc;
 
   if (wg == 0) {
@@ -684,9 +714,11 @@ tapgemm_f_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ C
       while (it.next(p, pc)) {
         const int ks = p.ksplit == 1 ? 0 : pc.rest % p.ksplit;
         const int nt = p.ksplit == 1 ? pc.rest : pc.rest / p.ksplit;
-        const int mtb = p.m_tiles_per_b == 1 ? pc.mt : pc.mt / p.m_tiles_per_b;
-        const int b0 = mtb * p.TB;
-        const int m0 = p.m_lo + (pc.mt - mtb * p.m_tiles_per_b) * p.TR;
+        const FTile t = f_tile(p, pc.mt);
+        const int b0 = t.b0, m0 = t.m0;
+        const CUtensorMap* mA0 = t.seg ? &tmA0s1 : &tmA0;
+        const CUtensorMap* mA1 = t.seg ? &tmA1s1 : &tmA1;
+        const uint32_t a_bytes = (uint32_t)t.TR * t.TB * 128u;     // the whole box: rows past the batch are zero-filled
         const int n0 = p.n_lo + nt * p.TN;
         // k-steps [kb, ke) of the tile's (tap, k-block) sequence; a split-K piece jumps to its first step.  An
         // interleaved k-split tile (ksplit > 1: the fc.0 GEMM, K = 16384) takes every ksplit-th (tap, k-block)
@@ -719,8 +751,8 @@ tapgemm_f_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ C
             mbar_wait(&ctl->empty[stage], phase ^ 1);
             uint8_t* sa = smem + stage * L::STAGE_BYTES;
             mbar_expect_tx(&ctl->full[stage], a_bytes + b_bytes);
-            if (k0 < p.a0_c) tma_load_3d(sa, &tmA0, &ctl->full[stage], k0, m0 + d + p.a_halo, b0);
-            else tma_load_3d(sa, &tmA1, &ctl->full[stage], k0 - p.a0_c, m0 + d + p.a_halo, b0);
+            if (k0 < p.a0_c) tma_load_3d(sa, mA0, &ctl->full[stage], k0, m0 + d + p.a_halo, b0);
+            else tma_load_3d(sa, mA1, &ctl->full[stage], k0 - p.a0_c, m0 + d + p.a_halo, b0);
             tma_load_2d(sa + A_STAGE_BYTES, &tmW, &ctl->full[stage], k0, (ti - p.w_tap0) * p.nc + n0);
             if (++stage == L::RING) { stage = 0; phase ^= 1; }
           }
@@ -790,8 +822,9 @@ tapgemm_f_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ C
     if (!partial) {
       if (p.tma_out) {
         const uint32_t buf = smem0 + L::STG_OFF + (uint32_t)(staged++ % L::BUFS) * L::BUF_BYTES;
-        f_epilogue_tma<TN>(p, acc, pc.mt, n0, ctid, buf, &tmO, &tmO2);
-      } else f_epilogue<TN>(p, acc, pc.mt, n0, ks, ctid, colstat);
+        const FTile t = f_tile(p, pc.mt);
+        f_epilogue_tma<TN>(p, acc, t, n0, ctid, buf, t.seg ? &tmOs1 : &tmO, &tmO2);
+      } else f_epilogue<TN>(p, acc, f_tile(p, pc.mt), n0, ks, ctid, colstat);
       if (tl_on && tl_i < TL_SLOTS - 1) tl[tl_i++] = gtime_ns();
       continue;
     }
@@ -822,7 +855,7 @@ tapgemm_f_tc(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ C
           acc[2 * j] += t.x; acc[2 * j + 1] += t.y;
         }
       }
-      f_epilogue<TN>(p, acc, pc.mt, n0, 0, ctid, colstat);
+      f_epilogue<TN>(p, acc, f_tile(p, pc.mt), n0, 0, ctid, colstat);
       __syncwarp();
       if ((ctid & 31) == 0) *cnt = 0u;             // ready for the next launch
       if (tl_on && tl_i < TL_SLOTS - 1) tl[tl_i++] = gtime_ns() | (1ull << 63);      // flagged: finisher
@@ -1098,14 +1131,46 @@ int tapgemm_f_tc_launch(const sg_tapgemm_f* q, cudaStream_t st) {
   p.batch = q->batch; p.ksplit = q->ksplit < 1 ? 1 : q->ksplit;
   const int rows_m = q->m_hi - q->m_lo;
   const int ncols = q->n_hi - q->n_lo;
-  if (rows_m >= 128) { p.TR = 128; p.TB = 1; }
-  else { p.TR = rows_m; p.TB = 128 / rows_m; if (p.TB > q->batch) p.TB = q->batch; }
-  p.m_tiles_per_b = (rows_m + p.TR - 1) / p.TR;
-  p.b_tiles = (q->batch + p.TB - 1) / p.TB;
   p.TN = (ncols % 256 == 0) ? 256 : (ncols % 128 == 0 ? 128 : 64);
   if ((q->tile_n == 64 || q->tile_n == 128 || q->tile_n == 256) && ncols % q->tile_n == 0 && q->tile_n < p.TN)
     p.TN = q->tile_n;      // narrow tiles: the caller split this launch off as the tail of a larger one
   p.n_tiles = ncols / p.TN;
+  // M tiling.  A segment of R rows per batch element is packed into 128-row tiles: TR = min(R, 128) rows of
+  // TB = min(128 / TR, batch) batch elements.  Row counts just above a multiple of 128 or of a power of two waste most
+  // of a tile (a data gradient computes R + 8 rows: 72 rows leave 56 of 128 dead, 264 rows a third tile of 8), so the
+  // rows may be split into a leading segment R0 (a multiple of 128, or the largest power of two <= rows_m) and the
+  // remaining R1 < 128 rows, packed on their own.  The split is taken when it strictly lowers the M tile count and
+  // still leaves at least one tile per SM: launches smaller than that (none of the step's at batch 300) keep their
+  // tiling and with it their stream-K tail.  out2 and BatchNorm-stat launches keep one segment: they compute a layer's
+  // own rows (powers of two in the step), and their second output and column statistics are written and tested with
+  // one segment only.
+  auto seg_tiles = [&](int R, int& TR, int& TB) {
+    if (R >= 128) { TR = 128; TB = 1; }
+    else { TR = R; TB = 128 / R; if (TB > q->batch) TB = q->batch; }
+    return ((R + TR - 1) / TR) * ((q->batch + TB - 1) / TB);
+  };
+  int R0 = rows_m;
+  p.m_tiles0 = seg_tiles(rows_m, p.TR, p.TB);
+  p.m_tiles = p.m_tiles0;
+  p.m_lo1 = q->m_hi; p.TR1 = 0; p.TB1 = 0;
+  if (q->out2 == nullptr && q->bn_stats == nullptr) {
+    int r0 = 128 * (rows_m / 128);
+    if (rows_m <= 128) for (r0 = 1; 2 * r0 <= rows_m; r0 *= 2) {}
+    if (r0 < rows_m) {
+      int TR0, TB0, TR1, TB1;
+      const int t0 = seg_tiles(r0, TR0, TB0), t1 = seg_tiles(rows_m - r0, TR1, TB1);
+      if (t0 + t1 < p.m_tiles && (t0 + t1) * p.n_tiles * p.ksplit >= num_sms()) {
+        R0 = r0;
+        p.TR = TR0; p.TB = TB0; p.m_tiles0 = t0; p.m_tiles = t0 + t1;
+        p.m_lo1 = q->m_lo + r0; p.TR1 = TR1; p.TB1 = TB1;
+      }
+    }
+  }
+  p.m_tiles_per_b = (R0 + p.TR - 1) / p.TR;
+  static const bool verbose = getenv("SEGAN_B200_SK_VERBOSE") != nullptr;
+  if (verbose)
+    fprintf(stderr, "tapgemm_f M tiles: %d rows x %d: %d rows as %d x %d -> %d, %d rows as %d x %d -> %d\n", rows_m,
+            q->batch, R0, p.TR, p.TB, p.m_tiles0, rows_m - R0, p.TR1, p.TB1, p.m_tiles - p.m_tiles0);
   {
     static const int dbg_env = [] { const char* e = getenv("SEGAN_B200_DEBUG"); return e ? atoi(e) : 0; }();
     p.dbg = dbg_env;
@@ -1123,9 +1188,17 @@ int tapgemm_f_tc_launch(const sg_tapgemm_f* q, cudaStream_t st) {
   if (q->a1) rc = make_map3(&tmA1, q->a1, q->a_dtype, q->a1_c, a_buf_rows, q->batch, p.TR, p.TB);
   else tmA1 = tmA0;
   if (rc) return rc;
+  CUtensorMap tmA0s1 = tmA0, tmA1s1 = tmA1;       // segment 1: the same rows, its own box
+  if (p.TR1 > 0) {
+    rc = make_map3(&tmA0s1, q->a0, q->a_dtype, q->a0_c, a_buf_rows, q->batch, p.TR1, p.TB1);
+    if (rc) return rc;
+    if (q->a1) rc = make_map3(&tmA1s1, q->a1, q->a_dtype, q->a1_c, a_buf_rows, q->batch, p.TR1, p.TB1);
+    else tmA1s1 = tmA0s1;
+    if (rc) return rc;
+  }
   rc = make_map2(&tmW, q->w, q->w_dtype, q->kc, (int64_t)(q->d_hi + 4 - q->w_tap0 + 1) * q->nc, p.TN);
   if (rc) return rc;
-  const int tiles = p.m_tiles_per_b * p.b_tiles * p.n_tiles * p.ksplit;
+  const int tiles = p.m_tiles * p.n_tiles * p.ksplit;
   int nctas = num_sms();
   if (tiles < nctas) nctas = tiles;
   // split-K over the last, partial wave (see PieceIter).  Cost model in k-steps of this launch's tile: leaving the
@@ -1147,7 +1220,6 @@ int tapgemm_f_tc_launch(const sg_tapgemm_f* q, cudaStream_t st) {
       if (c < best) { best = c; best_s = S; }
     }
     const bool split = best_s > 1 && best < 0.92 * steps && steps >= 2 * best_s;
-    static const bool verbose = getenv("SEGAN_B200_SK_VERBOSE") != nullptr;
     if (verbose)
       fprintf(stderr, "tapgemm_f split-K: %d tiles on %d CTAs, %d left over, %d k-steps, TN %d -> split %d\n",
               tiles, nctas, r, steps, p.TN, split ? best_s : 1);
@@ -1161,11 +1233,16 @@ int tapgemm_f_tc_launch(const sg_tapgemm_f* q, cudaStream_t st) {
   // whole tiles of a 16-bit output leave through shared memory and TMA stores (f_epilogue_tma); fp32 outputs (atomic
   // k-split, the waveform-end P), BatchNorm-stat launches and the split-K pieces store from the fragment
   p.tma_out = q->out_dtype != SG_F32 && q->bn_stats == nullptr;
-  CUtensorMap tmO = tmA0, tmO2 = tmA0;
+  CUtensorMap tmO = tmA0, tmO2 = tmA0, tmOs1 = tmA0;
   if (p.tma_out) {
-    rc = make_store_map3(&tmO, q->out, q->out_dtype, ncols, rows_m, q->batch, p.out_ld, q->out_rows + 2 * q->out_halo,
+    rc = make_store_map3(&tmO, q->out, q->out_dtype, ncols, R0, q->batch, p.out_ld, q->out_rows + 2 * q->out_halo,
                          q->out_halo + q->m_lo, p.out_col0, p.TR, p.TB);
     if (rc) return rc;
+    if (p.TR1 > 0) {
+      rc = make_store_map3(&tmOs1, q->out, q->out_dtype, ncols, rows_m - R0, q->batch, p.out_ld,
+                           q->out_rows + 2 * q->out_halo, q->out_halo + p.m_lo1, p.out_col0, p.TR1, p.TB1);
+      if (rc) return rc;
+    }
     if (q->out2 != nullptr) {
       rc = make_store_map3(&tmO2, q->out2, q->out_dtype, ncols, rows_m, q->batch, p.out_ld,
                            q->out_rows + 2 * q->out2_halo, q->out2_halo + q->m_lo, p.out_col0, p.TR, p.TB);
@@ -1173,13 +1250,14 @@ int tapgemm_f_tc_launch(const sg_tapgemm_f* q, cudaStream_t st) {
     }
   }
   const bool bf = q->a_dtype == SG_BF16;
-  void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, FTcParams);
+  void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap,
+               FTcParams);
   int smem_bytes;
   if (p.TN == 256) { kern = bf ? tapgemm_f_tc<256, true> : tapgemm_f_tc<256, false>; smem_bytes = FSmem<256>::BYTES; }
   else if (p.TN == 128) { kern = bf ? tapgemm_f_tc<128, true> : tapgemm_f_tc<128, false>; smem_bytes = FSmem<128>::BYTES; }
   else { kern = bf ? tapgemm_f_tc<64, true> : tapgemm_f_tc<64, false>; smem_bytes = FSmem<64>::BYTES; }
   SG_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-  void* args[] = {&tmA0, &tmA1, &tmW, &tmO, &tmO2, &p};
+  void* args[] = {&tmA0, &tmA1, &tmW, &tmO, &tmO2, &tmA0s1, &tmA1s1, &tmOs1, &p};
   SG_CHECK_CUDA(cudaLaunchKernel(reinterpret_cast<const void*>(kern), dim3(nctas), dim3(NUM_THREADS), args,
                                  (size_t)smem_bytes, st));
   return SG_OK;
