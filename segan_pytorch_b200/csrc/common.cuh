@@ -61,8 +61,10 @@ __device__ __forceinline__ float ld16(const void* p, int64_t i, int dtype) {
   if (dtype == SG_F16) return __half2float(reinterpret_cast<const __half*>(p)[i]);
   return __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p)[i]);
 }
+// fp16 stores saturate at +-65504 (a NaN stays NaN): a loss-scaled gradient that overflows clips instead of
+// turning into inf; bf16 has fp32's range
 __device__ __forceinline__ void st16(void* p, int64_t i, float v, int dtype) {
-  if (dtype == SG_F16) reinterpret_cast<__half*>(p)[i] = __float2half_rn(v);
+  if (dtype == SG_F16) reinterpret_cast<uint16_t*>(p)[i] = (uint16_t)pack_half2_sat(v, 0.f);
   else reinterpret_cast<__nv_bfloat16*>(p)[i] = __float2bfloat16_rn(v);
 }
 __device__ __forceinline__ uint16_t cvt16(float v, int dtype) {

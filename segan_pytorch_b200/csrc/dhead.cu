@@ -25,11 +25,6 @@ __device__ __forceinline__ float block_sum(float v, float* red /* [DHEAD_THREADS
   return t;
 }
 
-__device__ __forceinline__ void st_grad(void* p, int64_t i, float v, int dtype) {
-  if (dtype == SG_F16) v = fminf(fmaxf(v, -65504.f), 65504.f);     // loss-scaled fp16: clip instead of inf
-  st16(p, i, v, dtype);
-}
-
 __global__ void __launch_bounds__(DHEAD_THREADS)
 dhead_fwd_kernel(int pool_type, const __half* __restrict__ h, int Lq, int C, const float* __restrict__ pool_w,
                  const float* __restrict__ pool_b, const float* __restrict__ fc_w, const float* __restrict__ fc_b,
@@ -145,7 +140,7 @@ dhead_bwd_kernel(int pool_type, const __half* __restrict__ h, int batch, int Lq,
       float gw = 0.f;
       for (int t = 0; t < Lq; ++t) {
         const float ga = ga_s[t];
-        st_grad(g_h, gb + (int64_t)t * C + c, ga * w, gdt);
+        st16(g_h, gb + (int64_t)t * C + c, ga * w, gdt);
         if (g_pool_w) gw = fmaf(ga, __half2float(hb[(int64_t)t * C + c]), gw);
       }
       if (g_pool_w) atomicAdd(g_pool_w + c, gw);
@@ -157,10 +152,10 @@ dhead_bwd_kernel(int pool_type, const __half* __restrict__ h, int batch, int Lq,
     if (g_fc_w) atomicAdd(g_fc_w + c, gl * pooled[(int64_t)b * C + c]);
     if (pool_type == SG_DHEAD_GMAX) {
       const int idx = argmax[(int64_t)b * C + c];
-      for (int t = 0; t < Lq; ++t) st_grad(g_h, gb + (int64_t)t * C + c, t == idx ? gp : 0.f, gdt);
+      for (int t = 0; t < Lq; ++t) st16(g_h, gb + (int64_t)t * C + c, t == idx ? gp : 0.f, gdt);
     } else {
       const float g = gp / (float)Lq;
-      for (int t = 0; t < Lq; ++t) st_grad(g_h, gb + (int64_t)t * C + c, g, gdt);
+      for (int t = 0; t < Lq; ++t) st16(g_h, gb + (int64_t)t * C + c, g, gdt);
     }
   }
 }

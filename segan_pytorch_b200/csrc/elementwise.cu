@@ -1129,6 +1129,7 @@ extern "C" int sg_colsum(const void* a, int dtype, int64_t rows, int C, int mod,
 extern "C" int sg_fc_tail_fwd(const float* fc0_acc, const float* b0, const float* s1, const float* w2,
                               const float* b2, const float* s3, const float* w4, const float* b4, int batch,
                               float* z1, float* z2, float* logit, void* stream) {
+  SG_CHECK_ARG(batch > 0 && fc0_acc && b0 && s1 && w2 && b2 && s3 && w4 && b4 && z1 && z2 && logit);
   fc_tail_fwd_kernel<<<batch, 256, 0, ST>>>(fc0_acc, b0, s1, w2, b2, s3, w4, b4, z1, z2, logit);
   SG_CHECK_LAUNCH();
   return SG_OK;
@@ -1140,7 +1141,9 @@ extern "C" int sg_fc_tail_bwd(const float* z1, const float* z2, const float* log
                               float* loss_out, void* g_z1_bf16, float* ws /* [B*(1+128+256+256)] */, float* g_b0,
                               float* g_s1, float* g_w2, float* g_b2, float* g_s3, float* g_w4, float* g_b4,
                               float grad_scale, void* stream) {
-  SG_CHECK_ARG(ws && g_z1_bf16);
+  SG_CHECK_ARG(batch > 0 && z1 && z2 && logit && s1 && w2 && s3 && w4 && ws && g_z1_bf16);
+  // g_w2 == NULL skips the parameter gradients (the G step); otherwise the kernel adds into every one of them
+  SG_CHECK_ARG(!g_w2 || (g_b0 && g_s1 && g_b2 && g_s3 && g_w4 && g_b4));
   float* g_logit = ws;
   float* g_z2 = ws + batch;
   float* g_z1 = g_z2 + (int64_t)batch * FC2;
@@ -1160,6 +1163,7 @@ extern "C" int sg_fc_tail_bwd(const float* z1, const float* z2, const float* log
 
 extern "C" int sg_l1_loss_bwd(const float* y, const float* clean, int64_t n, float weight, float* loss_out,
                               float* gy, int accumulate, float grad_scale, void* stream) {
+  SG_CHECK_ARG(n > 0 && y && clean);
   reg_loss_bwd_kernel<REG_L1><<<REG_BLOCKS, 256, 0, ST>>>(y, clean, n, weight, loss_out, gy, accumulate, grad_scale);
   SG_CHECK_LAUNCH();
   return SG_OK;
@@ -1167,6 +1171,7 @@ extern "C" int sg_l1_loss_bwd(const float* y, const float* clean, int64_t n, flo
 
 extern "C" int sg_mse_loss_bwd(const float* y, const float* clean, int64_t n, float weight, float* loss_out,
                                float* gy, int accumulate, float grad_scale, void* stream) {
+  SG_CHECK_ARG(n > 0 && y && clean);
   reg_loss_bwd_kernel<REG_MSE><<<REG_BLOCKS, 256, 0, ST>>>(y, clean, n, weight, loss_out, gy, accumulate, grad_scale);
   SG_CHECK_LAUNCH();
   return SG_OK;

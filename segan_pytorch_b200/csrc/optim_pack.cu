@@ -425,8 +425,13 @@ __global__ void preemph_kernel(const float* __restrict__ x, int64_t n, float c, 
 using namespace sg;
 #define ST ((cudaStream_t)stream)
 
+// the kernels stream every buffer as float4: each must be 16-byte aligned
+static bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
 extern "C" int sg_rmsprop_step(float* param, float* grad, float* square_avg, int64_t n, float lr, float alpha,
                                float eps, float grad_scale, int clear_grad, void* stream) {
+  SG_CHECK_ARG(param && grad && square_avg && n >= 0);
+  SG_CHECK_ARG(aligned16(param) && aligned16(grad) && aligned16(square_avg));
   rmsprop_kernel<<<8 * NUM_SMS, 256, 0, ST>>>(param, grad, square_avg, n, lr, alpha, eps, grad_scale, clear_grad);
   SG_CHECK_LAUNCH();
   return SG_OK;
@@ -435,6 +440,9 @@ extern "C" int sg_rmsprop_step(float* param, float* grad, float* square_avg, int
 extern "C" int sg_adam_step(float* param, float* grad, float* exp_avg, float* exp_avg_sq, int64_t n, float lr,
                             float beta1, float beta2, float eps, int step, float grad_scale, int clear_grad,
                             void* stream) {
+  SG_CHECK_ARG(param && grad && exp_avg && exp_avg_sq && n >= 0);
+  SG_CHECK_ARG(aligned16(param) && aligned16(grad) && aligned16(exp_avg) && aligned16(exp_avg_sq));
+  SG_CHECK_ARG(step >= 1);                      // the bias corrections divide by 1 - beta^step
   const float bc1 = 1.f - powf(beta1, (float)step);
   const float bc2 = 1.f - powf(beta2, (float)step);
   adam_kernel<<<8 * NUM_SMS, 256, 0, ST>>>(param, grad, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps, bc1,
@@ -476,6 +484,8 @@ extern "C" int sg_unpack_wgrad(int kind, const float* dwp, int c_out, int c_in, 
                                const float* alpha, int alpha_from, float* dw, float* dalpha, int accumulate,
                                void* stream) {
   SG_CHECK_ARG(dwp && dw);
+  SG_CHECK_ARG(kind != 0 || (c_out % PO == 0 && c_in % PI == 0));     // the tile grid of sg_pack_weights
+  SG_CHECK_ARG(kind != 1 || (c_out % PI == 0 && c_in % PO == 0));
   static bool attr_set = false;
   if (!attr_set) {
     SG_CHECK_CUDA(cudaFuncSetAttribute(pack_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PACK_SMEM));

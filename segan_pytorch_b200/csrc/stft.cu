@@ -57,7 +57,10 @@ logpow_l1_kernel(const float* __restrict__ xg, const float* __restrict__ xc, int
     const float re = xg[r * ld + f], im = xg[r * ld + half + f];
     const float rc = xc[r * ld + f], ic = xc[r * ld + half + f];
     const float pg = re * re + im * im + 1e-19f, pc = rc * rc + ic * ic + 1e-19f;
-    const float d = k10 * (__logf(pg) - __logf(pc));            // 10 log10(pg) - 10 log10(pc)
+    // 10 log10(pg) - 10 log10(pc).  __fsub_rn keeps the subtraction out of an FMA with one logarithm's ln 2 scaling:
+    // contracted, identical powers would leave that product's rounding error as d != 0 and a full-size gradient of
+    // either sign where the reference's is 0
+    const float d = k10 * __fsub_rn(__logf(pg), __logf(pc));
     acc += fabsf(d);
     if (gx) {
       // d/d re [10 log10(re^2 + im^2 + eps)] = (20 / ln 10) re / p

@@ -99,8 +99,6 @@ __global__ void __launch_bounds__(256) tapgemm_f_ffma(FParams p) {
         float* dst = reinterpret_cast<float*>(p.out) + o;
         if (p.ksplit > 1) atomicAdd(dst, v);
         else *dst = v;
-      } else if (p.out_dtype == SG_F16) {
-        reinterpret_cast<uint16_t*>(p.out)[o] = (uint16_t)(pack_half2_sat(v, 0.f) & 0xffffu);
       } else {
         st16(p.out, o, v, p.out_dtype);
       }

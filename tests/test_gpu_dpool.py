@@ -122,6 +122,31 @@ def test_head_kernels_vs_torch(head, B, param_grads, grad_dtype):
         for got, ref, nm in zip(pg, grads[1:], ("pool_w", "pool_b", "fc_w", "fc_b")):
             if got is not None and ref is not None:
                 assert rel_err((got.cpu() - 0.5) / LS, ref) <= 1e-4, nm
+    # one more input: a given d loss / d logit with a NaN row and a row whose loss-scaled gradient is far past fp16's
+    # range -- g_h must hold NaN there and +-65504 (fp16; bf16: the value), never inf or a NaN clipped to a number
+    gx = torch.randn(B, y.numel() // B, generator=g)
+    gx[0] = float("nan")
+    if B > 1:
+        gx[1] = 1e6
+    hx = h.float().permute(0, 2, 1).contiguous().requires_grad_(True)
+    if conv:
+        px = F.conv1d(hx, pw.view(1, C_, 1), pb).view(B, Lq)
+    else:
+        px = (F.adaptive_max_pool1d if gmax else F.adaptive_avg_pool1d)(hx, 1).view(B, C_)
+    yx = px.reshape(-1) if mlp else F.linear(px, fw.view(1, -1), fb).view(-1)
+    ghx, = torch.autograd.grad((yx * gx.view(-1)).sum(), [hx])
+    g_hx = torch.zeros(B, Lq, C_, dtype=E.GT, device=DEV)
+    _lib.call("sg_dhead_bwd", kind, _p(hd), B, Lq, C_, _p(dpw) if conv else None, None if mlp else _p(dfw),
+              _p(pooled), _p(argmax), _p(logit), _p(gx.view(-1).to(DEV)), target, weight, None, _p(g_hx),
+              None, None, None, None, float(LS), _st())
+    torch.cuda.synchronize()
+    exp = ghx.permute(0, 2, 1) * LS
+    if E.GT == torch.float16:
+        exp = exp.clamp(-65504.0, 65504.0)
+    got = g_hx.float().cpu()
+    fin = ~torch.isnan(exp)
+    assert torch.equal(torch.isnan(got), ~fin) and not torch.isinf(got).any()
+    assert bool(((got[fin] - exp[fin]).abs() <= 8e-3 * exp[fin].abs() + 1e-4).all())
 
 
 def test_head_entry_points_reject_bad_arguments():

@@ -629,72 +629,8 @@ def test_bn_act_fwd_bwd(C_, L, roll, halo, variant, grad_dtype):
     assert rel_err(ga.float().permute(0, 2, 1).cpu(), an.grad) <= 1e-2
 
 
-def test_fc_tail_and_losses(grad_dtype):
-    g = _gen(7)
-    B = 6
-    acc = torch.randn(B, 256, generator=g).to(DEV)
-    b0, s1 = (0.1 * torch.randn(256, generator=g)).to(DEV), (0.25 * torch.ones(256)).to(DEV)
-    w2, b2 = (0.1 * torch.randn(128, 256, generator=g)).to(DEV), (0.1 * torch.randn(128, generator=g)).to(DEV)
-    s3 = (0.25 * torch.ones(128)).to(DEV)
-    w4, b4 = (0.1 * torch.randn(1, 128, generator=g)).to(DEV), torch.tensor([0.02], device=DEV)
-    z1, z2 = torch.zeros(B, 256, device=DEV), torch.zeros(B, 128, device=DEV)
-    logit = torch.zeros(B, 1, device=DEV)
-    _lib.call("sg_fc_tail_fwd", _p(acc), _p(b0), _p(s1), _p(w2), _p(b2), _p(s3), _p(w4), _p(b4), B, _p(z1), _p(z2),
-              _p(logit), _stream())
-    ps = [t.cpu().clone().requires_grad_(True) for t in (acc, b0, s1, w2, b2, s3, w4, b4)]
-    h = F.prelu(ps[0] + ps[1], ps[2])
-    h = F.prelu(F.linear(h, ps[3], ps[4]), ps[5])
-    ref = F.linear(h, ps[6], ps[7])
-    torch.cuda.synchronize()
-    assert max_abs(logit.cpu(), ref.detach()) <= 1e-5
-    loss = 0.5 * F.mse_loss(ref.view(-1), torch.ones(B))
-    loss.backward()
-    gz1 = torch.zeros(B, 256, dtype=E.GT, device=DEV)
-    ws = torch.zeros(B * 641, device=DEV)
-    gs = [torch.zeros_like(t) for t in (b0, s1, w2, b2, s3, w4, b4)]
-    lo = torch.zeros(1, device=DEV)
-    _lib.call("sg_fc_tail_bwd", _p(z1), _p(z2), _p(logit), None, 1.0, 0.5, _p(s1), _p(w2), _p(s3), _p(w4), B, _p(lo),
-              _p(gz1), _p(ws), *[_p(t) for t in gs], 8.0, _stream())
-    torch.cuda.synchronize()
-    assert abs(float(lo) - float(loss)) <= 1e-5                      # the loss itself is not scaled
-    assert rel_err(gz1.float().cpu() / 8.0, ps[0].grad) <= 1e-2      # grad_scale = 8 on every gradient
-    for got, p in zip(gs, ps[1:]):
-        assert rel_err(got.cpu().reshape(-1) / 8.0, p.grad.reshape(-1)) <= 1e-4
-    # L1
-    y, c = torch.randn(B, 64, generator=g).to(DEV), torch.randn(B, 64, generator=g).to(DEV)
-    gy = torch.zeros_like(y)
-    lo.zero_()
-    _lib.call("sg_l1_loss_bwd", _p(y), _p(c), y.numel(), 100.0, _p(lo), _p(gy), 0, 4.0, _stream())
-    yr = y.cpu().requires_grad_(True)
-    l = 100.0 * F.l1_loss(yr, c.cpu())
-    l.backward()
-    torch.cuda.synchronize()
-    assert abs(float(lo) - float(l)) <= 1e-3 and max_abs(gy.cpu() / 4.0, yr.grad) <= 1e-7
-
-
-def test_optimizers_and_emphasis():
+def test_deemphasis_and_preemphasis():
     g = _gen(8)
-    n = 10007
-    p0 = torch.randn(n, generator=g)
-    grads = [torch.randn(n, generator=g) for _ in range(3)]
-    for kind in ("rmsprop", "adam"):
-        pr = p0.clone().requires_grad_(True)
-        opt = torch.optim.RMSprop([pr], lr=5e-5) if kind == "rmsprop" else torch.optim.Adam([pr], lr=5e-5, betas=(0.0, 0.9))
-        p = p0.clone().to(DEV)
-        s1, s2 = torch.zeros(n, device=DEV), torch.zeros(n, device=DEV)
-        for t, gr in enumerate(grads, 1):
-            pr.grad = gr.clone()
-            opt.step()
-            gd = gr.to(DEV)
-            if kind == "rmsprop":
-                _lib.call("sg_rmsprop_step", _p(p), _p(gd), _p(s1), n, 5e-5, 0.99, 1e-8, 1.0, t % 2, _stream())
-            else:
-                _lib.call("sg_adam_step", _p(p), _p(gd), _p(s1), _p(s2), n, 5e-5, 0.0, 0.9, 1e-8, t, 1.0, t % 2, _stream())
-            torch.cuda.synchronize()
-            # clear_grad: the gradient is zeroed as it is read (odd steps here), left alone otherwise
-            assert (int(gd.count_nonzero()) == 0) == (t % 2 == 1)
-        torch.cuda.synchronize()
-        assert max_abs(p.cpu(), pr.detach()) <= 2e-7, kind
     y = (0.1 * torch.randn(50001, generator=g))
     x = torch.zeros_like(y).to(DEV)
     _lib.call("sg_deemphasis", _p(y.to(DEV)), y.numel(), 0.95, _p(x), _stream())
@@ -836,85 +772,6 @@ def test_generator_forward_fused_vs_unfused_activation():
         finally:
             E.FUSE_ACT = prev
     assert max_abs(outs[0], outs[1]) <= 3e-4
-
-
-# ------------------------------------------------------------------------------------------------------
-# round 2: packed-master path (emit operands / alpha gradient / folds) against the tensor-algebra twins
-# ------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("kind,co,ci,tl", [(0, 128, 64, 0), (1, 64, 256, 0), (2, 256, 128, 16)])
-def test_packed_master_roundtrip_and_operands(kind, co, ci, tl):
-    """sg_pack_weights(-> fp32 master) / sg_unpack_wgrad(alpha None) == engine.pack_reference / unpack_reference, and
-    sg_emit_operands produces exactly the operands the reference-layout packer (sg_pack_weights, 16-bit) makes."""
-    g = _gen(31)
-    shape = (co, ci, 31) if kind == 0 else ((ci, co, 31) if kind == 1 else (co, ci * tl))
-    w = torch.randn(*shape, generator=g).to(DEV)
-    layer = E.PackedLayer("w", kind, co, ci, tl, "f", "dg", alpha_name="alpha" if kind == 1 else None)
-    m = torch.zeros(layer.numel, device=DEV)
-    _lib.call("sg_pack_weights", kind, _p(w), co, ci, tl, None, 0, _p(m), None, SG_F32, SG_F32, _stream())
-    torch.cuda.synchronize()
-    ref = E.pack_reference(kind, w.cpu(), co, ci, tl)
-    assert torch.equal(m.cpu().view(ref.shape), ref)
-    back = torch.zeros_like(w)
-    _lib.call("sg_unpack_wgrad", kind, _p(m), co, ci, tl, None, None, 0, _p(back), None, 0, _stream())
-    torch.cuda.synchronize()
-    assert torch.equal(back, w)
-    # operands: from the master (new path) vs from the reference layout (round-1 path)
-    alpha = (0.5 + torch.rand(ci // 2, generator=g)).to(DEV) if kind == 1 else None
-    T, nc, kc = layer.T, layer.nc, layer.kc
-    f1 = torch.zeros(T, nc, kc, dtype=torch.float16, device=DEV)
-    d1 = torch.zeros(T, kc, nc, dtype=torch.float16, device=DEV)
-    f0, d0 = torch.zeros_like(f1), torch.zeros_like(d1)
-    _lib.call("sg_emit_operands", _p(m), T, nc, kc, _p(alpha), ci // 2 if kind == 1 else 0, _p(f1), _p(d1), SG_F16, SG_F16,
-              None, _stream())
-    _lib.call("sg_pack_weights", kind, _p(w), co, ci, tl, _p(alpha), ci // 2, _p(f0), _p(d0), SG_F16, SG_F16, _stream())
-    torch.cuda.synchronize()
-    assert torch.equal(f1, f0) and torch.equal(d1, d0)
-
-
-def test_alpha_grad_and_folds():
-    """sg_alpha_grad == what sg_unpack_wgrad(alpha) computes (dW = alpha*dWeff on the skip half, dalpha = sum dWeff*W);
-    the waveform-end folds against their index formulas (and they clear what they read)."""
-    g = _gen(32)
-    co, ci = 64, 256
-    w = torch.randn(ci, co, 31, generator=g).to(DEV)
-    dweff_ref_layout = torch.randn(ci, co, 31, generator=g)
-    alpha = (0.5 + torch.rand(ci // 2, generator=g)).to(DEV)
-    m = E.pack_reference(1, w.cpu(), co, ci, 0).to(DEV).contiguous()
-    dwp = E.pack_reference(1, dweff_ref_layout, co, ci, 0).to(DEV).contiguous()
-    dalpha = torch.zeros(ci // 2, device=DEV)
-    _lib.call("sg_alpha_grad", _p(dwp), _p(m), 9, 4 * co, ci, _p(alpha), ci // 2, _p(dalpha), _stream())
-    torch.cuda.synchronize()
-    dw = E.unpack_reference(1, dwp.cpu().view(9, 4 * co, ci), co, ci, 0)
-    exp = dweff_ref_layout.clone()
-    exp[ci // 2:] *= alpha.cpu().view(-1, 1, 1)
-    assert rel_err(dw, exp) <= 1e-6
-    assert rel_err(dalpha.cpu(), (dweff_ref_layout[ci // 2:] * w.cpu()[ci // 2:]).sum((1, 2))) <= 1e-5
-    # first conv fold, cin = 2
-    dwq = torch.randn(2, 64, 2, 64, generator=g).to(DEV)
-    src = dwq.cpu().clone()
-    dwg = torch.ones(64, 2, 31, device=DEV)
-    _lib.call("sg_wave_wgrad_fold", _p(dwq), 2, _p(dwg), _stream())
-    torch.cuda.synchronize()
-    exp = 1 + (src[0, :, 0, :] + src[1, :, 1, :]).view(64, 2, 32)[:, :, :31]
-    assert rel_err(dwg.cpu(), exp) <= 1e-6
-    after = dwq.cpu().view(2, 64, 2, 2, 32)
-    assert float(after[0, :, 0, :, :31].abs().max()) == 0.0 and float(after[1, :, 1, :, :31].abs().max()) == 0.0
-    assert torch.equal(after[0, :, 1], src.view(2, 64, 2, 2, 32)[0, :, 1])          # off-diagonal blocks untouched
-    # last deconv fold
-    half = 64
-    dwq = torch.randn(2, 64, 2, 2, half, generator=g).to(DEV)
-    src = dwq.cpu().clone()
-    wl = torch.randn(2 * half, 1, 31, generator=g).to(DEV)
-    al = (0.5 + torch.rand(half, generator=g)).to(DEV)
-    gw = torch.zeros(2 * half, 1, 31, device=DEV)
-    ga = torch.zeros(half, device=DEV)
-    _lib.call("sg_last_deconv_wgrad_fold", _p(dwq), half, _p(wl), _p(al), _p(gw), _p(ga), _stream())
-    torch.cuda.synchronize()
-    dweff = (src[0, :, :, 0, :] + src[1, :, :, 1, :]).permute(1, 2, 0).reshape(2 * half, 64)[:, :31]
-    exp = dweff.clone()
-    exp[half:] *= al.cpu().view(-1, 1)
-    assert rel_err(gw.cpu()[:, 0], exp) <= 1e-6
-    assert rel_err(ga.cpu(), (dweff[half:] * wl.cpu()[half:, 0]).sum(1)) <= 1e-5
 
 
 @pytest.mark.parametrize("B,L,kind", [(3, 16384, "speech"), (2, 4096, "white"), (5, 16384, "weak_hf")])

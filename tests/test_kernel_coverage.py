@@ -12,9 +12,6 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 # entry point -> the GPU test that checks it through a wrapper (its name does not appear in the test itself)
 EXEMPT = {
     "sg_tapgemm_w_run": "tests/test_gpu_tapgemm_w.py::test_tapgemm_w_vs_fp64 (through engine.run_w)",
-    "sg_stft_frames": "tests/test_gpu_kernels.py::test_spectral_loss_gemm_vs_torch_stft (through engine.SpectralLoss)",
-    "sg_stft_frames_fold": "tests/test_gpu_kernels.py::test_spectral_loss_gemm_vs_torch_stft (through engine.SpectralLoss)",
-    "sg_logpow_l1": "tests/test_gpu_kernels.py::test_spectral_loss_gemm_vs_torch_stft (through engine.SpectralLoss)",
 }
 
 
