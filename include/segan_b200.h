@@ -217,6 +217,14 @@ int sg_pack_weights(int kind, const float* w, int c_out, int c_in, int t_len,
 int sg_unpack_wgrad(int kind, const float* dwp, int c_out, int c_in, int t_len,
                     const float* w, const float* alpha, int alpha_from,
                     float* dw, float* dalpha, int accumulate, void* stream);
+/* The same for kernel width kw (4 <= kw <= 32; ignored for kind 2): W[..][..][kw], tap index 4d + p + kw/2 - 1
+ * (Conv1d) and -4d + r + (kw - 4)/2 (ConvTranspose1d); the entry points above are these with kw = 31. */
+int sg_pack_weights_kw(int kind, const float* w, int c_out, int c_in, int t_len, int kw,
+                       const float* alpha, int alpha_from,
+                       void* w_fwd, void* w_dgrad, int dtype_fwd, int dtype_dgrad, void* stream);
+int sg_unpack_wgrad_kw(int kind, const float* dwp, int c_out, int c_in, int t_len, int kw,
+                       const float* w, const float* alpha, int alpha_from,
+                       float* dw, float* dalpha, int accumulate, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Waveform-end layers (Cin or Cout in {1,2}: HBM-bound, CUDA cores).
@@ -253,12 +261,18 @@ int sg_wave_deconv_bwd(const void* x0, int c0, const void* x1, int c1, int batch
  * tap-GEMMs with K = 64; the transposed forms are a GEMM followed by a shift-add. */
 int sg_wave_im2col(const float* v0, const float* v1, int cin, int batch, int L, int roll, const int32_t* roll_dev,
                    int reflect, int off, void* col_f16, void* col_bf16, void* stream);
+/* the same for kernel width kw (4 <= kw <= 32): columns k >= kw are zero (sg_wave_im2col: kw = 31) */
+int sg_wave_im2col_kw(const float* v0, const float* v1, int cin, int batch, int L, int roll, const int32_t* roll_dev,
+                      int reflect, int off, int kw, void* col_f16, void* col_bf16, void* stream);
 /* y[b][4m+r] = tanh(bias + sum_d P[b][m+d][(d+4)*4+r]); P fp32 [B][Lin][64] (last decoder block) */
 int sg_wave_shiftadd_tanh(const float* P, int batch, int Lin, const float* bias, float* y, void* stream);
 /* gx[b][unroll(reflect(q))] += sum_{4t+k-14=q} P2[b][t][col0+k]; P2 bf16 [B][L/4][64] (D input gradient;
  * col0 = 32*ci selects the input channel) */
 int sg_wave_col2im_fold(const void* P2, int col0, int batch, int L, int roll, const int32_t* roll_dev, float* gx,
                         void* stream);
+/* the same for kernel width kw (4 <= kw <= 32): sum over k < kw of 4t+k-(kw/2-1) = q (sg_wave_col2im_fold: kw = 31) */
+int sg_wave_col2im_fold_kw(const void* P2, int col0, int batch, int L, int roll, const int32_t* roll_dev, int kw,
+                           float* gx, void* stream);
 /* gpre = gy*(1-y^2); dbias += sum(gpre) */
 int sg_tanh_bwd(const float* gy, const float* y, int64_t n, float* gpre, float* dbias, void* stream);
 
@@ -426,6 +440,11 @@ int sg_last_deconv_wgrad_fold(float* dwq /* the blocks read are cleared */, int 
 /* the same fold for a Generator without skips (skip=False): dwq[2][64][2][cin] (s, k-slot, s', c) -> dW[cin][1][31]
  * += dwq[0][k][0][c] + dwq[1][k][1][c]; no alpha */
 int sg_last_deconv_wgrad_fold_1src(float* dwq /* the blocks read are cleared */, int cin, float* dw, void* stream);
+/* the three folds for kernel width kw (4 <= kw <= 32): k-slots k < kw, dw [..][..][kw] (the entry points above: kw = 31) */
+int sg_wave_wgrad_fold_kw(float* dwq, int cin, int kw, float* dw, void* stream);
+int sg_last_deconv_wgrad_fold_kw(float* dwq, int half, int kw, const float* w, const float* alpha, float* dw,
+                                 float* dalpha, void* stream);
+int sg_last_deconv_wgrad_fold_1src_kw(float* dwq, int cin, int kw, float* dw, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Convolutional skip connection (GSkip skip_type='conv', generator.py:43-49): nn.Conv1d(C, C, K, stride 1,

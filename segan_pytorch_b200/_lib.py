@@ -90,6 +90,13 @@ _SIGS = {
     "sg_wave_wgrad_fold": [_vp, _i, _vp, _vp],
     "sg_last_deconv_wgrad_fold": [_vp, _i, _vp, _vp, _vp, _vp, _vp],
     "sg_last_deconv_wgrad_fold_1src": [_vp, _i, _vp, _vp],
+    "sg_pack_weights_kw": [_i, _vp, _i, _i, _i, _i, _vp, _i, _vp, _vp, _i, _i, _vp],
+    "sg_unpack_wgrad_kw": [_i, _vp, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _i, _vp],
+    "sg_wave_im2col_kw": [_vp, _vp, _i, _i, _i, _i, _vp, _i, _i, _i, _vp, _vp, _vp],
+    "sg_wave_col2im_fold_kw": [_vp, _i, _i, _i, _i, _vp, _i, _vp, _vp],
+    "sg_wave_wgrad_fold_kw": [_vp, _i, _i, _vp, _vp],
+    "sg_last_deconv_wgrad_fold_kw": [_vp, _i, _i, _vp, _vp, _vp, _vp, _vp],
+    "sg_last_deconv_wgrad_fold_1src_kw": [_vp, _i, _i, _vp, _vp],
     "sg_deemphasis": [_vp, _i64, _f, _vp, _vp],
     "sg_preemphasis": [_vp, _i64, _f, _vp, _vp],
     "sg_pcm16_to_wave": [_vp, _vp, _i64, _i, _f, _vp, _vp, _vp],

@@ -43,6 +43,10 @@ extern int g_grad_dtype;
   } while (0)
 
 constexpr int KW = 31;      // kernel width (train.opts gkwidth)
+// served kernel widths of the stride-4 layers (engine.KW_MIN / KW_MAX): the waveform-end im2col holds 32 taps per
+// input channel; below 4 a stride-4 transposed conv does not give 4x its input
+constexpr int KW_MIN = 4, KW_MAX = 32;
+__host__ __device__ __forceinline__ bool kw_served(int kw) { return kw >= KW_MIN && kw <= KW_MAX; }
 constexpr int NTAP = 9;     // row taps d in [-4, 4] of the stride-1 "row" formulation
 constexpr int NUM_SMS = 132;    // H100 SXM
 

@@ -93,33 +93,37 @@ adam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
 }
 
 // ------------------------------------------------------------------------------------------
-// packing.  One block handles a 16 x 16 (outer x inner channel) tile of the fp32 master and all
-// 31 taps: coalesced 496-float reads, 32-byte segment writes into both packed layouts.
+// packing.  One block handles a 16 x 32 (outer x inner channel) tile of the fp32 master and all
+// kw taps: coalesced reads, 32-byte segment writes into both packed layouts.
 //
-// kind 0 (Conv1d W[co][ci][k]):
-//   Wf [d+4][co][p*Cin + ci] = W[co][ci][ 4d + p + 14]        (fwd:   K = (p,ci), N = co)
-//   Wdg[d+4][p*Cin + ci][co] = W[co][ci][-4d + p + 14]        (dgrad: K = co, N = (p,ci))
-// kind 1 (ConvTranspose1d W[ci][co][k], alpha folded for ci >= alpha_from):
-//   Wt [d+4][r*Cout + co][ci] = a(ci) W[ci][co][-4d + r + 13] (fwd:   K = ci, N = (r,co))
-//   Wtd[d+4][ci][r*Cout + co] = a(ci) W[ci][co][ 4d + r + 13] (dgrad: K = (r,co), N = ci)
-// entries whose tap index falls outside [0, 30] are zero.
+// kind 0 (Conv1d W[co][ci][k], reflect pad kw/2 - 1 on the left: o = kw/2 - 1, 14 for kw = 31):
+//   Wf [d+4][co][p*Cin + ci] = W[co][ci][ 4d + p + o]         (fwd:   K = (p,ci), N = co)
+//   Wdg[d+4][p*Cin + ci][co] = W[co][ci][-4d + p + o]         (dgrad: K = co, N = (p,ci))
+// kind 1 (ConvTranspose1d W[ci][co][k], padding P = (kw - 4)/2, 13 for kw = 31; alpha folded for ci >= alpha_from):
+//   Wt [d+4][r*Cout + co][ci] = a(ci) W[ci][co][-4d + r + P]  (fwd:   K = ci, N = (r,co))
+//   Wtd[d+4][ci][r*Cout + co] = a(ci) W[ci][co][ 4d + r + P]  (dgrad: K = (r,co), N = ci)
+// entries whose tap index falls outside [0, kw) are zero.  4 <= kw <= 32: with at most 32 taps every index
+// 4d + p + o (|d| <= 4) of a stride-4 layer lies within the 9-tap table.
 // ------------------------------------------------------------------------------------------
-constexpr int PO = 16, PI = 32;              // tile: 16 outer x 32 inner channels x 31 taps (3 CTAs/SM)
+constexpr int PO = 16, PI = 32;              // tile: 16 outer x 32 inner channels x kw taps (3 CTAs/SM)
 constexpr int PACK_THREADS = 512;
-constexpr int PACK_SMEM = PO * PI * (KW + 2) * 4;   // last dim padded to 33 words: conflict-free transposes
+constexpr int PACK_SMEM = PO * PI * (KW_MAX + 1) * 4;   // last dim padded to 33 words: conflict-free transposes
+
+__host__ __device__ __forceinline__ int tap_offset(int kind, int kw) { return kind == 0 ? kw / 2 - 1 : (kw - 4) / 2; }
 
 __global__ void __launch_bounds__(PACK_THREADS)
-pack_conv_kernel(int kind, const float* __restrict__ w, int c_outer, int c_inner, const float* __restrict__ alpha,
+pack_conv_kernel(int kind, int kw, const float* __restrict__ w, int c_outer, int c_inner, const float* __restrict__ alpha,
                  int alpha_from, void* __restrict__ w_fwd, void* __restrict__ w_dg, int dt_fwd, int dt_dg) {
-  // master layout is [outer][inner][31]; kind 0: outer = co, inner = ci ; kind 1: outer = ci, inner = co
+  // master layout is [outer][inner][kw]; kind 0: outer = co, inner = ci ; kind 1: outer = ci, inner = co
   extern __shared__ float tile_raw[];
-  float (*tile)[PI][KW + 2] = reinterpret_cast<float (*)[PI][KW + 2]>(tile_raw);
+  float (*tile)[PI][KW_MAX + 1] = reinterpret_cast<float (*)[PI][KW_MAX + 1]>(tile_raw);
   const int o0 = blockIdx.y * PO, i0 = blockIdx.x * PI;
   const int tid = threadIdx.x;
-  for (int idx = tid; idx < PO * PI * KW; idx += PACK_THREADS) {
-    const int oo = idx / (PI * KW), rem = idx % (PI * KW);
-    const int ii = rem / KW, k = rem % KW;
-    float v = w[((int64_t)(o0 + oo) * c_inner + (i0 + ii)) * KW + k];
+  const int off = tap_offset(kind, kw);
+  for (int idx = tid; idx < PO * PI * kw; idx += PACK_THREADS) {
+    const int oo = idx / (PI * kw), rem = idx % (PI * kw);
+    const int ii = rem / kw, k = rem % kw;
+    float v = w[((int64_t)(o0 + oo) * c_inner + (i0 + ii)) * kw + k];
     if (kind == 1 && alpha && (o0 + oo) >= alpha_from) v *= alpha[o0 + oo - alpha_from];
     tile[oo][ii][k] = v;
   }
@@ -129,26 +133,26 @@ pack_conv_kernel(int kind, const float* __restrict__ w, int c_outer, int c_inner
     {  // A: lo = inner
       const int lo = idx % PI, hi = (idx / PI) % PO, ph = (idx / (PI * PO)) % 4, ti = idx / (4 * PI * PO);
       const int d = ti - 4;
-      if (kind == 0) {   // Wf[ti][co = hi][ph*Cin + ci = lo],  k = 4d + ph + 14
-        const int k = 4 * d + ph + 14;
-        const float v = (k >= 0 && k < KW) ? tile[hi][lo][k] : 0.f;
+      if (kind == 0) {   // Wf[ti][co = hi][ph*Cin + ci = lo],  k = 4d + ph + o
+        const int k = 4 * d + ph + off;
+        const float v = (k >= 0 && k < kw) ? tile[hi][lo][k] : 0.f;
         if (w_fwd) st_any(w_fwd, ((int64_t)ti * c_outer + (o0 + hi)) * (4 * c_inner) + ph * c_inner + (i0 + lo), v, dt_fwd);
-      } else {           // Wtd[ti][ci = hi][ph*Cout + co = lo],  k = 4d + ph + 13
-        const int k = 4 * d + ph + 13;
-        const float v = (k >= 0 && k < KW) ? tile[hi][lo][k] : 0.f;
+      } else {           // Wtd[ti][ci = hi][ph*Cout + co = lo],  k = 4d + ph + P
+        const int k = 4 * d + ph + off;
+        const float v = (k >= 0 && k < kw) ? tile[hi][lo][k] : 0.f;
         if (w_dg) st_any(w_dg, ((int64_t)ti * c_outer + (o0 + hi)) * (4 * c_inner) + ph * c_inner + (i0 + lo), v, dt_dg);
       }
     }
     {  // B: lo = outer
       const int lo = idx % PO, hi = (idx / PO) % PI, ph = (idx / (PI * PO)) % 4, ti = idx / (4 * PI * PO);
       const int d = ti - 4;
-      if (kind == 0) {   // Wdg[ti][ph*Cin + ci = hi][co = lo],  k = -4d + ph + 14
-        const int k = -4 * d + ph + 14;
-        const float v = (k >= 0 && k < KW) ? tile[lo][hi][k] : 0.f;
+      if (kind == 0) {   // Wdg[ti][ph*Cin + ci = hi][co = lo],  k = -4d + ph + o
+        const int k = -4 * d + ph + off;
+        const float v = (k >= 0 && k < kw) ? tile[lo][hi][k] : 0.f;
         if (w_dg) st_any(w_dg, ((int64_t)ti * (4 * c_inner) + ph * c_inner + (i0 + hi)) * c_outer + (o0 + lo), v, dt_dg);
-      } else {           // Wt[ti][ph*Cout + co = hi][ci = lo],  k = -4d + ph + 13
-        const int k = -4 * d + ph + 13;
-        const float v = (k >= 0 && k < KW) ? tile[lo][hi][k] : 0.f;
+      } else {           // Wt[ti][ph*Cout + co = hi][ci = lo],  k = -4d + ph + P
+        const int k = -4 * d + ph + off;
+        const float v = (k >= 0 && k < kw) ? tile[lo][hi][k] : 0.f;
         if (w_fwd) st_any(w_fwd, ((int64_t)ti * (4 * c_inner) + ph * c_inner + (i0 + hi)) * c_outer + (o0 + lo), v, dt_fwd);
       }
     }
@@ -172,17 +176,18 @@ __global__ void pack_fc_kernel(const float* __restrict__ w, int nout, int C, int
 
 // ------------------------------------------------------------------------------------------
 // unpack: packed fp32 dWp -> reference layout
-// kind 0: dW[co][ci][k] = dWf[d+4][co][p*Cin+ci],  k = 4d + p + 14
-// kind 1: dWe[ci][co][k] = dWt[d+4][r*Cout+co][ci], k = -4d + r + 13 ; dW = a(ci) dWe ;
+// kind 0: dW[co][ci][k] = dWf[d+4][co][p*Cin+ci],  k = 4d + p + o
+// kind 1: dWe[ci][co][k] = dWt[d+4][r*Cout+co][ci], k = -4d + r + P ; dW = a(ci) dWe ;
 //         dalpha[ci-alpha_from] = sum_{co,k} dWe * W
 // kind 2: dW[n][c*T+t] = dW1p[n][t*C+c]
 // ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(PACK_THREADS)
-unpack_conv_kernel(int kind, const float* __restrict__ dwp, int c_outer, int c_inner, const float* __restrict__ w,
+unpack_conv_kernel(int kind, int kw, const float* __restrict__ dwp, int c_outer, int c_inner, const float* __restrict__ w,
                    const float* __restrict__ alpha, int alpha_from, float* __restrict__ dw,
                    float* __restrict__ dalpha, int accumulate) {
   extern __shared__ float tile_raw[];
-  float (*tile)[PI][KW + 2] = reinterpret_cast<float (*)[PI][KW + 2]>(tile_raw);
+  float (*tile)[PI][KW_MAX + 1] = reinterpret_cast<float (*)[PI][KW_MAX + 1]>(tile_raw);
+  const int off = tap_offset(kind, kw);
   __shared__ float ared[PO];
   const int o0 = blockIdx.y * PO, i0 = blockIdx.x * PI;
   const int tid = threadIdx.x;
@@ -190,22 +195,22 @@ unpack_conv_kernel(int kind, const float* __restrict__ dwp, int c_outer, int c_i
   for (int idx = tid; idx < NTAP * 4 * PO * PI; idx += PACK_THREADS) {
     if (kind == 0) {   // dWf[ti][co = hi][ph*Cin + ci = lo]: contiguous along the inner channel
       const int lo = idx % PI, hi = (idx / PI) % PO, ph = (idx / (PI * PO)) % 4, ti = idx / (4 * PI * PO);
-      const int k = 4 * (ti - 4) + ph + 14;
-      if (k >= 0 && k < KW)
+      const int k = 4 * (ti - 4) + ph + off;
+      if (k >= 0 && k < kw)
         tile[hi][lo][k] = dwp[((int64_t)ti * c_outer + (o0 + hi)) * (4 * c_inner) + ph * c_inner + (i0 + lo)];
     } else {           // dWt[ti][ph*Cout + co = hi][ci = lo]: contiguous along the outer channel
       const int lo = idx % PO, hi = (idx / PO) % PI, ph = (idx / (PI * PO)) % 4, ti = idx / (4 * PI * PO);
-      const int k = -4 * (ti - 4) + ph + 13;
-      if (k >= 0 && k < KW)
+      const int k = -4 * (ti - 4) + ph + off;
+      if (k >= 0 && k < kw)
         tile[lo][hi][k] = dwp[((int64_t)ti * (4 * c_inner) + ph * c_inner + (i0 + hi)) * c_outer + (o0 + lo)];
     }
   }
   __syncthreads();
-  // PI*KW = 992 consecutive master elements share one outer channel `oo`
+  // PI*kw consecutive master elements share one outer channel `oo`
   for (int oo = 0; oo < PO; ++oo) {
-    for (int e = tid; e < PI * KW; e += PACK_THREADS) {
-      const int ii = e / KW, k = e % KW;
-      const int64_t gi = ((int64_t)(o0 + oo) * c_inner + (i0 + ii)) * KW + k;
+    for (int e = tid; e < PI * kw; e += PACK_THREADS) {
+      const int ii = e / kw, k = e % kw;
+      const int64_t gi = ((int64_t)(o0 + oo) * c_inner + (i0 + ii)) * kw + k;
       float v = tile[oo][ii][k];
       float contrib = 0.f;
       const bool al = kind == 1 && alpha && (o0 + oo) >= alpha_from;
@@ -300,14 +305,15 @@ alpha_grad_kernel(float* __restrict__ dwp, const float* __restrict__ m, int64_t 
 }
 
 // Waveform-end layer gradients out of their single-tap GEMM results (both tiny):
-//   first conv (Cin = 1 | 2): dwq[2][64][2][64] (position-pair s x co x pair s' x (ci*32 + k)); the s == s' blocks
-//   are the gradient:  dW[co][ci][k] += dwq[0][co][0][ci*32+k] + dwq[1][co][1][ci*32+k]
-//   (the blocks read are zeroed again: dwq needs no fill before the next weight-gradient GEMM accumulates into it)
-__global__ void wave_wgrad_fold_kernel(float* __restrict__ dwq, int cin, float* __restrict__ dw) {
+//   first conv (Cin = 1 | 2, width kw): dwq[2][64][2][64] (position-pair s x co x pair s' x (ci*32 + k)); the s == s'
+//   blocks are the gradient:  dW[co][ci][k] += dwq[0][co][0][ci*32+k] + dwq[1][co][1][ci*32+k],  k < kw
+//   (the blocks read are zeroed again: dwq needs no fill before the next weight-gradient GEMM accumulates into it;
+//   the im2col columns k >= kw are zero, so the GEMM leaves the columns not read here at zero)
+__global__ void wave_wgrad_fold_kernel(float* __restrict__ dwq, int cin, int kw, float* __restrict__ dw) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= 64 * cin * KW) return;
-  const int co = i / (cin * KW), rem = i % (cin * KW);
-  const int ci = rem / KW, k = rem % KW;
+  if (i >= 64 * cin * kw) return;
+  const int co = i / (cin * kw), rem = i % (cin * kw);
+  const int ci = rem / kw, k = rem % kw;
   const int col = ci * 32 + k;
   float* p0 = dwq + ((0 * 64 + co) * 2 + 0) * 64 + col;
   float* p1 = dwq + ((1 * 64 + co) * 2 + 1) * 64 + col;
@@ -316,25 +322,25 @@ __global__ void wave_wgrad_fold_kernel(float* __restrict__ dwq, int cin, float* 
   *p1 = 0.f;
   atomicAdd(dw + i, v);
 }
-//   last deconv (Cout = 1, alpha folded into its effective weight): dwq[2][64][NSRC][2][half] (s, k-slot, source,
-//   s', c); dWeff[src*half + c][k] = dwq[0][k][src][0][c] + dwq[1][k][src][1][c]; dW += dWeff (* alpha for the skip
+//   last deconv (Cout = 1, width kw, alpha folded into its effective weight): dwq[2][64][NSRC][2][half] (s, k-slot,
+//   source, s', c); dWeff[src*half + c][k] = dwq[0][k][src][0][c] + dwq[1][k][src][1][c], k < kw; dW += dWeff (* alpha for the skip
 //   half), dalpha[c] += sum_k dWeff[half + c][k] * W[half + c][k].  NSRC = 2: cat(decoder, skip); NSRC = 1: the
 //   decoder output alone (no skips: no alpha, w / alpha / dalpha unused)
 template <int NSRC>
-__global__ void last_deconv_wgrad_fold_kernel(float* __restrict__ dwq, int half, const float* __restrict__ w,
+__global__ void last_deconv_wgrad_fold_kernel(float* __restrict__ dwq, int half, int kw, const float* __restrict__ w,
                                               const float* __restrict__ alpha, float* __restrict__ dw,
                                               float* __restrict__ dalpha) {
   const int ch = blockIdx.x * blockDim.x + threadIdx.x;       // channel of cat(decoder, skip): [0, NSRC*half)
   if (ch >= NSRC * half) return;
   const int src = ch / half, c = ch % half;
   float da = 0.f;
-  for (int k = 0; k < KW; ++k) {
+  for (int k = 0; k < kw; ++k) {
     float* p0 = dwq + ((((int64_t)0 * 64 + k) * NSRC + src) * 2 + 0) * half + c;
     float* p1 = dwq + ((((int64_t)1 * 64 + k) * NSRC + src) * 2 + 1) * half + c;
     const float v = *p0 + *p1;
     *p0 = 0.f;
     *p1 = 0.f;
-    const int64_t wi = (int64_t)ch * KW + k;
+    const int64_t wi = (int64_t)ch * kw + k;
     if (NSRC == 2 && src == 1) {
       da = fmaf(v, w[wi], da);
       atomicAdd(dw + wi, v * alpha[c]);
@@ -451,10 +457,10 @@ extern "C" int sg_adam_step(float* param, float* grad, float* exp_avg, float* ex
   return SG_OK;
 }
 
-extern "C" int sg_pack_weights(int kind, const float* w, int c_out, int c_in, int t_len, const float* alpha,
-                               int alpha_from, void* w_fwd, void* w_dgrad, int dtype_fwd, int dtype_dgrad,
-                               void* stream) {
-  SG_CHECK_ARG(w && (w_fwd || w_dgrad));
+extern "C" int sg_pack_weights_kw(int kind, const float* w, int c_out, int c_in, int t_len, int kw,
+                                  const float* alpha, int alpha_from, void* w_fwd, void* w_dgrad, int dtype_fwd,
+                                  int dtype_dgrad, void* stream) {
+  SG_CHECK_ARG(w && (w_fwd || w_dgrad) && (kind == 2 || kw_served(kw)));
   static bool attr_set = false;
   if (!attr_set) {
     SG_CHECK_CUDA(cudaFuncSetAttribute(pack_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PACK_SMEM));
@@ -464,13 +470,13 @@ extern "C" int sg_pack_weights(int kind, const float* w, int c_out, int c_in, in
   if (kind == 0) {
     SG_CHECK_ARG(c_out % PO == 0 && c_in % PI == 0);
     dim3 grid(c_in / PI, c_out / PO);
-    pack_conv_kernel<<<grid, PACK_THREADS, PACK_SMEM, ST>>>(0, w, c_out, c_in, nullptr, 0, w_fwd, w_dgrad, dtype_fwd,
-                                                   dtype_dgrad);
+    pack_conv_kernel<<<grid, PACK_THREADS, PACK_SMEM, ST>>>(0, kw, w, c_out, c_in, nullptr, 0, w_fwd, w_dgrad,
+                                                            dtype_fwd, dtype_dgrad);
   } else if (kind == 1) {
     SG_CHECK_ARG(c_out % PI == 0 && c_in % PO == 0);
     dim3 grid(c_out / PI, c_in / PO);
-    pack_conv_kernel<<<grid, PACK_THREADS, PACK_SMEM, ST>>>(1, w, c_in, c_out, alpha, alpha_from, w_fwd, w_dgrad, dtype_fwd,
-                                                   dtype_dgrad);
+    pack_conv_kernel<<<grid, PACK_THREADS, PACK_SMEM, ST>>>(1, kw, w, c_in, c_out, alpha, alpha_from, w_fwd, w_dgrad,
+                                                            dtype_fwd, dtype_dgrad);
   } else if (kind == 2) {
     pack_fc_kernel<<<4 * NUM_SMS, 256, 0, ST>>>(w, c_out, c_in, t_len, w_fwd, w_dgrad, dtype_fwd, dtype_dgrad);
   } else {
@@ -480,10 +486,17 @@ extern "C" int sg_pack_weights(int kind, const float* w, int c_out, int c_in, in
   return SG_OK;
 }
 
-extern "C" int sg_unpack_wgrad(int kind, const float* dwp, int c_out, int c_in, int t_len, const float* w,
-                               const float* alpha, int alpha_from, float* dw, float* dalpha, int accumulate,
+extern "C" int sg_pack_weights(int kind, const float* w, int c_out, int c_in, int t_len, const float* alpha,
+                               int alpha_from, void* w_fwd, void* w_dgrad, int dtype_fwd, int dtype_dgrad,
                                void* stream) {
-  SG_CHECK_ARG(dwp && dw);
+  return sg_pack_weights_kw(kind, w, c_out, c_in, t_len, 31, alpha, alpha_from, w_fwd, w_dgrad, dtype_fwd, dtype_dgrad,
+                            stream);
+}
+
+extern "C" int sg_unpack_wgrad_kw(int kind, const float* dwp, int c_out, int c_in, int t_len, int kw, const float* w,
+                                  const float* alpha, int alpha_from, float* dw, float* dalpha, int accumulate,
+                                  void* stream) {
+  SG_CHECK_ARG(dwp && dw && (kind == 2 || kw_served(kw)));
   SG_CHECK_ARG(kind != 0 || (c_out % PO == 0 && c_in % PI == 0));     // the tile grid of sg_pack_weights
   SG_CHECK_ARG(kind != 1 || (c_out % PI == 0 && c_in % PO == 0));
   static bool attr_set = false;
@@ -494,12 +507,12 @@ extern "C" int sg_unpack_wgrad(int kind, const float* dwp, int c_out, int c_in, 
   }
   if (kind == 0) {
     dim3 grid(c_in / PI, c_out / PO);
-    unpack_conv_kernel<<<grid, PACK_THREADS, PACK_SMEM, ST>>>(0, dwp, c_out, c_in, nullptr, nullptr, 0, dw, nullptr,
-                                                     accumulate);
+    unpack_conv_kernel<<<grid, PACK_THREADS, PACK_SMEM, ST>>>(0, kw, dwp, c_out, c_in, nullptr, nullptr, 0, dw, nullptr,
+                                                              accumulate);
   } else if (kind == 1) {
     dim3 grid(c_out / PI, c_in / PO);
-    unpack_conv_kernel<<<grid, PACK_THREADS, PACK_SMEM, ST>>>(1, dwp, c_in, c_out, w, alpha, alpha_from, dw, dalpha,
-                                                     accumulate);
+    unpack_conv_kernel<<<grid, PACK_THREADS, PACK_SMEM, ST>>>(1, kw, dwp, c_in, c_out, w, alpha, alpha_from, dw, dalpha,
+                                                              accumulate);
   } else if (kind == 2) {
     unpack_fc_kernel<<<4 * NUM_SMS, 256, 0, ST>>>(dwp, c_out, c_in, t_len, dw, accumulate);
   } else {
@@ -507,6 +520,12 @@ extern "C" int sg_unpack_wgrad(int kind, const float* dwp, int c_out, int c_in, 
   }
   SG_CHECK_LAUNCH();
   return SG_OK;
+}
+
+extern "C" int sg_unpack_wgrad(int kind, const float* dwp, int c_out, int c_in, int t_len, const float* w,
+                               const float* alpha, int alpha_from, float* dw, float* dalpha, int accumulate,
+                               void* stream) {
+  return sg_unpack_wgrad_kw(kind, dwp, c_out, c_in, t_len, 31, w, alpha, alpha_from, dw, dalpha, accumulate, stream);
 }
 
 extern "C" int sg_emit_operands(const float* master, int n_taps, int nc, int kc, const float* alpha, int alpha_from,
@@ -534,26 +553,39 @@ extern "C" int sg_alpha_grad(float* dwp, const float* master, int n_taps, int nc
   return SG_OK;
 }
 
+extern "C" int sg_wave_wgrad_fold_kw(float* dwq, int cin, int kw, float* dw, void* stream) {
+  SG_CHECK_ARG(dwq && dw && (cin == 1 || cin == 2) && kw_served(kw));
+  wave_wgrad_fold_kernel<<<(64 * cin * kw + 255) / 256, 256, 0, ST>>>(dwq, cin, kw, dw);
+  SG_CHECK_LAUNCH();
+  return SG_OK;
+}
+
 extern "C" int sg_wave_wgrad_fold(float* dwq, int cin, float* dw, void* stream) {
-  SG_CHECK_ARG(dwq && dw && (cin == 1 || cin == 2));
-  wave_wgrad_fold_kernel<<<(64 * cin * KW + 255) / 256, 256, 0, ST>>>(dwq, cin, dw);
+  return sg_wave_wgrad_fold_kw(dwq, cin, 31, dw, stream);
+}
+
+extern "C" int sg_last_deconv_wgrad_fold_kw(float* dwq, int half, int kw, const float* w, const float* alpha,
+                                            float* dw, float* dalpha, void* stream) {
+  SG_CHECK_ARG(dwq && w && alpha && dw && half > 0 && kw_served(kw));
+  last_deconv_wgrad_fold_kernel<2><<<(2 * half + 127) / 128, 128, 0, ST>>>(dwq, half, kw, w, alpha, dw, dalpha);
   SG_CHECK_LAUNCH();
   return SG_OK;
 }
 
 extern "C" int sg_last_deconv_wgrad_fold(float* dwq, int half, const float* w, const float* alpha, float* dw,
                                          float* dalpha, void* stream) {
-  SG_CHECK_ARG(dwq && w && alpha && dw && half > 0);
-  last_deconv_wgrad_fold_kernel<2><<<(2 * half + 127) / 128, 128, 0, ST>>>(dwq, half, w, alpha, dw, dalpha);
+  return sg_last_deconv_wgrad_fold_kw(dwq, half, 31, w, alpha, dw, dalpha, stream);
+}
+
+extern "C" int sg_last_deconv_wgrad_fold_1src_kw(float* dwq, int cin, int kw, float* dw, void* stream) {
+  SG_CHECK_ARG(dwq && dw && cin > 0 && kw_served(kw));
+  last_deconv_wgrad_fold_kernel<1><<<(cin + 127) / 128, 128, 0, ST>>>(dwq, cin, kw, nullptr, nullptr, dw, nullptr);
   SG_CHECK_LAUNCH();
   return SG_OK;
 }
 
 extern "C" int sg_last_deconv_wgrad_fold_1src(float* dwq, int cin, float* dw, void* stream) {
-  SG_CHECK_ARG(dwq && dw && cin > 0);
-  last_deconv_wgrad_fold_kernel<1><<<(cin + 127) / 128, 128, 0, ST>>>(dwq, cin, nullptr, nullptr, dw, nullptr);
-  SG_CHECK_LAUNCH();
-  return SG_OK;
+  return sg_last_deconv_wgrad_fold_1src_kw(dwq, cin, 31, dw, stream);
 }
 
 extern "C" int sg_deemphasis(const float* y, int64_t n, float coef, float* x, void* stream) {

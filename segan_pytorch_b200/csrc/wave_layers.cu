@@ -331,11 +331,11 @@ extern "C" int sg_wave_deconv_bwd(const void* x0, int c0, const void* x1, int c1
 // ==========================================================================================
 namespace sg {
 
-// col[b][t][ci*32 + k] = pad(v_ci)[4t + k - off]   (k < 31; k = 31 and absent channels = 0)
+// col[b][t][ci*32 + k] = pad(v_ci)[4t + k - off]   (k < kw <= 32; columns k >= kw and absent channels = 0)
 __global__ void __launch_bounds__(256)
 wave_im2col_kernel(const float* __restrict__ v0, const float* __restrict__ v1, int cin, int batch, int L, int roll,
                    const int* __restrict__ roll_dev,
-                   int mode, int off, void* __restrict__ col_f16, void* __restrict__ col_bf16) {
+                   int mode, int off, int kw, void* __restrict__ col_f16, void* __restrict__ col_bf16) {
   if (roll_dev) roll = *roll_dev;
   const int Lq = L / 4;
   const int64_t total = (int64_t)batch * Lq * 8;
@@ -350,7 +350,7 @@ wave_im2col_kernel(const float* __restrict__ v0, const float* __restrict__ v1, i
     for (int j = 0; j < 8; ++j) {
       const int k = k0 + j;
       float x = 0.f;
-      if (ci < cin && k < KW) x = wave_at(v, (int64_t)b * L, 4 * t + k - off, L, mode, roll);
+      if (ci < cin && k < kw) x = wave_at(v, (int64_t)b * L, 4 * t + k - off, L, mode, roll);
       o16.v[j] = cvt16(x, SG_F16);
       ob.v[j] = cvt16(x, SG_BF16);
     }
@@ -366,7 +366,7 @@ wave_im2col_kernel(const float* __restrict__ v0, const float* __restrict__ v1, i
 constexpr int IM2_T = 256;
 __global__ void __launch_bounds__(256)
 wave_im2col_tiled_kernel(const float* __restrict__ v0, const float* __restrict__ v1, int cin, int L, int roll,
-                         const int* __restrict__ roll_dev, int mode, int off, uint16_t* __restrict__ col_f16,
+                         const int* __restrict__ roll_dev, int mode, int off, int kw, uint16_t* __restrict__ col_f16,
                          uint16_t* __restrict__ col_bf16) {
   constexpr int SEG = 4 * IM2_T + 32;            // input samples one tile touches (4 t + k, k < 32), padded
   __shared__ float xs[2][SEG + 4];
@@ -386,7 +386,7 @@ wave_im2col_tiled_kernel(const float* __restrict__ v0, const float* __restrict__
     const int ci = seg >> 2, k0 = (seg & 3) * 8;
     float x[8];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) x[j] = (ci < cin && k0 + j < KW) ? xs[ci][4 * r + k0 + j] : 0.f;
+    for (int j = 0; j < 8; ++j) x[j] = (ci < cin && k0 + j < kw) ? xs[ci][4 * r + k0 + j] : 0.f;
     const int64_t o = ((int64_t)b * Lq + t0 + r) * 64 + seg * 8;
     if (col_f16) {
       uint32_t w[4];
@@ -429,24 +429,25 @@ wave_shiftadd_tanh_kernel(const float* __restrict__ P, int batch, int Lin, const
   }
 }
 
-// gx[b][src(q)] += sum_{t,k: 4t + k - 14 = q} P2[b][t][k]   (reflect fold + un-roll), P2 16-bit (gradient dtype) [B][Lq][64]
+// gx[b][src(q)] += sum_{t,k < kw: 4t + k - off = q} P2[b][t][k]   (reflect fold + un-roll), P2 16-bit (gradient
+// dtype) [B][Lq][64]; off = kw/2 - 1 is the left reflect pad, the right one is off + 1
 __global__ void __launch_bounds__(256)
 wave_col2im_fold_kernel(const void* __restrict__ P2, int gdt, int col0, int batch, int L, int roll,
-                        const int* __restrict__ roll_dev, float* __restrict__ gx) {
+                        const int* __restrict__ roll_dev, int off, int kw, float* __restrict__ gx) {
   if (roll_dev) roll = *roll_dev;
   const int Lq = L / 4;
-  const int span = L + 30;                         // q in [-14, L + 15]
+  const int span = L + 2 * off + 2;                // q in [-off, L + off + 1]
   const int64_t total = (int64_t)batch * span;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-    const int q = (int)(i % span) - 14;
+    const int q = (int)(i % span) - off;
     const int b = (int)(i / span);
-    const int e = q + 14;                          // = 4t + k
+    const int e = q + off;                         // = 4t + k
     float s = 0.f;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const int k = (e & 3) + 4 * j;
       const int t = (e - k) / 4;
-      if (k < KW && t >= 0 && t < Lq) s += ld16(P2, ((int64_t)b * Lq + t) * 64 + col0 + k, gdt);
+      if (k < kw && t >= 0 && t < Lq) s += ld16(P2, ((int64_t)b * Lq + t) * 64 + col0 + k, gdt);
     }
     const int src = unroll_idx(reflect_idx(q, L), roll, L);
     atomicAdd(gx + (int64_t)b * L + src, s);
@@ -455,14 +456,14 @@ wave_col2im_fold_kernel(const void* __restrict__ P2, int gdt, int col0, int batc
 
 }  // namespace sg
 
-extern "C" int sg_wave_im2col(const float* v0, const float* v1, int cin, int batch, int L, int roll,
-                              const int32_t* roll_dev, int reflect,
-                              int off, void* col_f16, void* col_bf16, void* stream) {
-  SG_CHECK_ARG(v0 && (cin == 1 || (cin == 2 && v1)) && L % 4 == 0 && (col_f16 || col_bf16));
+extern "C" int sg_wave_im2col_kw(const float* v0, const float* v1, int cin, int batch, int L, int roll,
+                                 const int32_t* roll_dev, int reflect, int off, int kw, void* col_f16, void* col_bf16,
+                                 void* stream) {
+  SG_CHECK_ARG(v0 && (cin == 1 || (cin == 2 && v1)) && L % 4 == 0 && (col_f16 || col_bf16) && kw_served(kw));
   if (batch <= 65535) {
     dim3 grid((unsigned)cdiv(L / 4, IM2_T), (unsigned)batch);
     wave_im2col_tiled_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(
-        v0, v1, cin, L, roll, roll_dev, reflect ? PAD_REFLECT : PAD_ZERO, off, reinterpret_cast<uint16_t*>(col_f16),
+        v0, v1, cin, L, roll, roll_dev, reflect ? PAD_REFLECT : PAD_ZERO, off, kw, reinterpret_cast<uint16_t*>(col_f16),
         reinterpret_cast<uint16_t*>(col_bf16));
     SG_CHECK_LAUNCH();
     return SG_OK;
@@ -471,9 +472,16 @@ extern "C" int sg_wave_im2col(const float* v0, const float* v1, int cin, int bat
   int64_t g = cdiv(total, 256 * 4);
   if (g > 16 * NUM_SMS) g = 16 * NUM_SMS;
   wave_im2col_kernel<<<(int)g, 256, 0, (cudaStream_t)stream>>>(v0, v1, cin, batch, L, roll, roll_dev,
-                                                              reflect ? PAD_REFLECT : PAD_ZERO, off, col_f16, col_bf16);
+                                                              reflect ? PAD_REFLECT : PAD_ZERO, off, kw, col_f16,
+                                                              col_bf16);
   SG_CHECK_LAUNCH();
   return SG_OK;
+}
+
+extern "C" int sg_wave_im2col(const float* v0, const float* v1, int cin, int batch, int L, int roll,
+                              const int32_t* roll_dev, int reflect,
+                              int off, void* col_f16, void* col_bf16, void* stream) {
+  return sg_wave_im2col_kw(v0, v1, cin, batch, L, roll, roll_dev, reflect, off, KW, col_f16, col_bf16, stream);
 }
 
 extern "C" int sg_wave_shiftadd_tanh(const float* P, int batch, int Lin, const float* bias, float* y, void* stream) {
@@ -485,14 +493,22 @@ extern "C" int sg_wave_shiftadd_tanh(const float* P, int batch, int Lin, const f
   return SG_OK;
 }
 
-extern "C" int sg_wave_col2im_fold(const void* P2, int col0, int batch, int L, int roll, const int32_t* roll_dev,
-                                   float* gx, void* stream) {
-  const int64_t total = (int64_t)batch * (L + 30);
+extern "C" int sg_wave_col2im_fold_kw(const void* P2, int col0, int batch, int L, int roll, const int32_t* roll_dev,
+                                      int kw, float* gx, void* stream) {
+  SG_CHECK_ARG(P2 && gx && kw_served(kw));
+  const int off = kw / 2 - 1;
+  const int64_t total = (int64_t)batch * (L + 2 * off + 2);
   int64_t g = cdiv(total, 256 * 4);
   if (g > 16 * NUM_SMS) g = 16 * NUM_SMS;
-  wave_col2im_fold_kernel<<<(int)g, 256, 0, (cudaStream_t)stream>>>(P2, g_grad_dtype, col0, batch, L, roll, roll_dev, gx);
+  wave_col2im_fold_kernel<<<(int)g, 256, 0, (cudaStream_t)stream>>>(P2, g_grad_dtype, col0, batch, L, roll, roll_dev,
+                                                                    off, kw, gx);
   SG_CHECK_LAUNCH();
   return SG_OK;
+}
+
+extern "C" int sg_wave_col2im_fold(const void* P2, int col0, int batch, int L, int roll, const int32_t* roll_dev,
+                                   float* gx, void* stream) {
+  return sg_wave_col2im_fold_kw(P2, col0, batch, L, roll, roll_dev, KW, gx, stream);
 }
 
 // gpre = gy * (1 - y^2), dbias += sum gpre   (tanh backward of the last decoder block)

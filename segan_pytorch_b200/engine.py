@@ -4,8 +4,9 @@ PyTorch is used for device memory (caching allocator), streams and parameter sto
 FLOP of the hot path runs in libsegan_b200.so through the C ABI (segan_pytorch_b200._lib).
 
 Layer geometry follows the reference (file:line into santi-pdp/segan_pytorch):
-  encoder block  = reflect-pad(14,15) -> Conv1d(k31,s4) -> [BatchNorm1d] -> PReLU   segan/models/modules.py:91-105
-  decoder block  = ConvTranspose1d(k31,s4,p13)[:-1] -> PReLU | Tanh                 segan/models/modules.py:135-141
+  encoder block  = reflect-pad(k//2-1,k//2) -> Conv1d(k,s4) -> [BatchNorm1d] -> PReLU   segan/models/modules.py:91-105
+  decoder block  = ConvTranspose1d(k,s4,p=(k-4)//2)[:-1 if k odd] -> PReLU | Tanh     segan/models/modules.py:135-141
+                   (k = 31 in SEGAN+; every width 4 <= k <= 32 is served, see kwidth_served)
   G wiring       = 5 enc -> cat(z, h) -> 5 x (cat(h, alpha*skip), dec)              segan/models/generator.py:180-230
                    (no_z: h alone into dec 0; skip=False: every dec block reads h alone)
   D wiring       = 5 x (phase shift, enc with BN) -> FC 16384-256-128-1             segan/models/discriminator.py:150-194
@@ -22,7 +23,27 @@ from . import _lib
 from ._lib import (ACT_NONE, ACT_PRELU, BACKEND_FFMA, BACKEND_TCGEN05, SG_BF16, SG_DHEAD_CONV, SG_DHEAD_GAVG,
                    SG_DHEAD_GMAX, SG_DHEAD_MLP, SG_F16, SG_F32, TapGemmF, TapGemmW)
 
-KW = 31
+# Kernel widths of the stride-4 convs and transposed convs: activations are rows of 4 positions with a 16-position
+# halo, so a width-k layer is a 9-tap (d = -4..4) GEMM over those rows for every k <= 35.  The bound 32 is the
+# waveform-end layers' im2col (32 columns per input channel); below 4 the reference's transposed conv does not give
+# 4 * Lin samples, so its skip concat fails.
+KW_MIN, KW_MAX = 4, 32
+
+
+def kwidth_served(k):
+    return isinstance(k, int) and not isinstance(k, bool) and KW_MIN <= k <= KW_MAX
+
+
+def conv_offset(k):
+    """Left reflect pad of a width-k encoder conv (modules.py:94-97): tap index = 4d + p + conv_offset(k)."""
+    return k // 2 - 1
+
+
+def deconv_padding(k):
+    """Padding of a width-k stride-4 ConvTranspose1d (modules.py:116): tap index = -4d + r + deconv_padding(k)."""
+    return max(0, (4 - k) // -2)
+
+
 # Discriminator pool_type -> head kernel selector of sg_dhead_fwd / _bwd ('none' runs fc.0 + sg_fc_tail instead)
 DHEAD_KINDS = {"conv": SG_DHEAD_CONV, "gmax": SG_DHEAD_GMAX, "gavg": SG_DHEAD_GAVG, "mlp": SG_DHEAD_MLP}
 
@@ -33,26 +54,27 @@ def wave_on_tensor_cores():
 
 
 def wave_col_weights(w, dev):
-    """Conv1d weight [64][cin][31] -> single-tap operand Wcol[co][ci*32 + k] (fp32, [64][64])."""
+    """Conv1d weight [64][cin][k] -> single-tap operand Wcol[co][ci*32 + j] = W[co][ci][j] for j < k (fp32, [64][64])."""
     wc = torch.zeros(w.shape[0], 2, 32, dtype=torch.float32, device=dev)
-    wc[:, :w.shape[1], :KW] = w
+    wc[:, :w.shape[1], :w.shape[2]] = w
     return wc.view(w.shape[0], 64)
 
 
-_DEC_LAST_KIDX = None
+_DEC_LAST_KIDX = {}
 
 
-def dec_last_tap_index(dev):
-    """jj = (d+4)*4 + r  ->  k = -4d + r + 13 (or -1): column order of the last decoder block's GEMM."""
-    global _DEC_LAST_KIDX
-    if _DEC_LAST_KIDX is None or _DEC_LAST_KIDX.device != dev:
+def dec_last_tap_index(dev, k=31):
+    """jj = (d+4)*4 + r  ->  j = -4d + r + deconv_padding(k) (or -1 outside [0, k)): column order of the last decoder
+    block's GEMM for a width-k transposed conv."""
+    key = (dev, k)
+    if key not in _DEC_LAST_KIDX:
         idx = []
         for jj in range(64):
             d, r = jj // 4 - 4, jj % 4
-            k = -4 * d + r + 13
-            idx.append(k if (jj < 36 and 0 <= k < KW) else -1)
-        _DEC_LAST_KIDX = torch.tensor(idx, device=dev)
-    return _DEC_LAST_KIDX
+            j = -4 * d + r + deconv_padding(k)
+            idx.append(j if (jj < 36 and 0 <= j < k) else -1)
+        _DEC_LAST_KIDX[key] = torch.tensor(idx, device=dev)
+    return _DEC_LAST_KIDX[key]
 
 
 def default_backend():
@@ -138,25 +160,45 @@ def _require_cuda(*ts):
 # --------------------------------------------------------------------------------------------
 # structural-zero tap ranges of the four packed weight layouts
 # --------------------------------------------------------------------------------------------
-def tap_ranges(kind, c, kc, nc):
+def _phase_span(kind, d, k):
+    """Stride phases (lo, hi inclusive) that forward tap d of a width-k layer reads, or None: conv phase p holds tap
+    index 4d + p + conv_offset(k), deconv phase r holds -4d + r + deconv_padding(k); valid indices are [0, k)."""
+    if kind == "conv":
+        ph = [p for p in range(4) if 0 <= 4 * d + p + conv_offset(k) < k]
+    else:
+        ph = [r for r in range(4) if 0 <= -4 * d + r + deconv_padding(k) < k]
+    return (ph[0], ph[-1]) if ph else None
+
+
+def tap_ranges(kind, c, kc, nc, k=31):
     """kind: conv_fwd | conv_dgrad | deconv_fwd | deconv_dgrad | full ; c = the channel count whose
-    four stride phases are interleaved (Cin for conv, Cout for deconv)."""
+    four stride phases are interleaved (Cin for conv, Cout for deconv); k = the kernel width.  Blocks of phases a tap
+    does not read are structurally zero in the packed weight and are skipped; a tap that reads none gets an empty
+    range (tap_span gives the d_lo, d_hi of the others).  k = 31: d=-4 reads conv phases {2,3} / deconv phases
+    {0,1}, d=+4 conv phase 0 / deconv phase 3."""
     k_lo, k_hi, n_lo, n_hi = [0] * 9, [kc] * 9, [0] * 9, [nc] * 9
-    if kind == "conv_fwd":        # K = (p, ci): d=-4 -> p in {2,3}; d=+4 -> p = 0
-        k_lo[0], k_hi[0] = 2 * c, 4 * c
-        k_lo[8], k_hi[8] = 0, c
-    elif kind == "conv_dgrad":    # N = (p, ci): d=-4 -> p = 0; d=+4 -> p in {2,3}
-        n_lo[0], n_hi[0] = 0, c
-        n_lo[8], n_hi[8] = 2 * c, 4 * c
-    elif kind == "deconv_fwd":    # N = (r, co): d=-4 -> r in {0,1}; d=+4 -> r = 3
-        n_lo[0], n_hi[0] = 0, 2 * c
-        n_lo[8], n_hi[8] = 3 * c, 4 * c
-    elif kind == "deconv_dgrad":  # K = (r, co): d=-4 -> r = 3; d=+4 -> r in {0,1}
-        k_lo[0], k_hi[0] = 3 * c, 4 * c
-        k_lo[8], k_hi[8] = 0, 2 * c
-    elif kind != "full":
+    if kind == "full":
+        return k_lo, k_hi, n_lo, n_hi
+    if kind not in ("conv_fwd", "conv_dgrad", "deconv_fwd", "deconv_dgrad"):
         raise ValueError(kind)
+    base, form = kind.split("_")
+    # the data-gradient operand's tap d is the transpose of the forward tap -d: its phases move to the other side
+    on_k = (base == "conv") == (form == "fwd")          # conv_fwd / deconv_dgrad: phases are K; else N
+    lo, hi = (k_lo, k_hi) if on_k else (n_lo, n_hi)
+    for i in range(9):
+        d = i - 4 if form == "fwd" else 4 - i
+        span = _phase_span(base, d, k)
+        if span is None:
+            lo[i], hi[i] = 0, 0
+        elif span != (0, 3):
+            lo[i], hi[i] = span[0] * c, (span[1] + 1) * c
     return k_lo, k_hi, n_lo, n_hi
+
+
+def tap_span(taps):
+    """(d_lo, d_hi) of the non-empty taps of a tap table (they are contiguous for every width >= 4)."""
+    live = [i - 4 for i in range(9) if taps[1][i] > taps[0][i] and taps[3][i] > taps[2][i]]
+    return live[0], live[-1]
 
 
 # optional live profiling (bench.py): list of (kind, start_event, end_event, algorithmic_flops)
@@ -487,17 +529,18 @@ def grad_twins():
 class PackedLayer(object):
     """One tap-GEMM layer whose fp32 master, optimiser state and gradient live in the layout of its forward
     operand, M[T][nc][kc] (include/segan_b200.h "Packed-master path").
-      kind 0: Conv1d W[cout][cin][31]          -> M[9][cout][4cin]
-      kind 1: ConvTranspose1d W[cin][cout][31] -> M[9][4cout][cin]   (alpha: GSkip scale of the columns >= alpha_from)
+      kind 0: Conv1d W[cout][cin][kw]          -> M[9][cout][4cin]
+      kind 1: ConvTranspose1d W[cin][cout][kw] -> M[9][4cout][cin]   (alpha: GSkip scale of the columns >= alpha_from)
       kind 2: Linear W[nout][C*T]              -> M[1][nout][T*C]"""
 
-    def __init__(self, name, kind, c_out, c_in, t_len, f_key, dg_key, alpha_name=None, tied=False):
+    def __init__(self, name, kind, c_out, c_in, t_len, f_key, dg_key, alpha_name=None, tied=False, kw=31):
         """tied (skip_merge='sum', generator.py:72-74): W (hi + alpha*skip) = [W | alpha W] cat(hi, skip) -- the
         layer runs as the two-source concat GEMM over 2*Cin' input channels whose two halves hold the SAME weights:
         `c_in` is the doubled count, import duplicates the parameter, export returns the first half, and the
         gradients of the two halves are summed into both (finish_grads) so the copies never drift apart."""
         self.name, self.kind, self.c_out, self.c_in, self.t_len = name, kind, c_out, c_in, t_len
         self.f_key, self.dg_key, self.alpha_name, self.tied = f_key, dg_key, alpha_name, tied
+        self.kw = kw
         if kind == 0:
             self.T, self.nc, self.kc = 9, c_out, 4 * c_in
         elif kind == 1:
@@ -509,24 +552,34 @@ class PackedLayer(object):
         self.off = 0
 
 
-def pack_reference(kind, w, c_out, c_in, t_len):
-    """Reference layout -> packed master layout M[T][nc][kc], as tensor algebra (host-side twin of sg_pack_weights:
-    used for CPU-resident modules -- optimiser state dicts, checkpoints -- and as the kernels' cross-check)."""
-    if kind == 0:        # M[d+4][co][p*Cin+ci] = W[co][ci][4d+p+14]
-        wp = torch.nn.functional.pad(w.reshape(c_out, c_in, KW), (2, 3))
+def _tap_pad(kind, k):
+    """Left zero pad that places the k taps of a width-k weight in the 36 = 9 x 4 (tap, phase) slots."""
+    return 16 - (conv_offset(k) if kind == 0 else deconv_padding(k))
+
+
+def pack_reference(kind, w, c_out, c_in, t_len, k=31):
+    """Reference layout -> packed master layout M[T][nc][kc], as tensor algebra (host-side twin of sg_pack_weights_kw:
+    used for CPU-resident modules -- optimiser state dicts, checkpoints -- and as the kernels' cross-check).
+    k = kernel width of kinds 0 and 1."""
+    if kind == 0:        # M[d+4][co][p*Cin+ci] = W[co][ci][4d+p+conv_offset(k)]
+        lp = _tap_pad(0, k)
+        wp = torch.nn.functional.pad(w.reshape(c_out, c_in, k), (lp, 36 - k - lp))
         return wp.view(c_out, c_in, 9, 4).permute(2, 0, 3, 1).reshape(9, c_out, 4 * c_in).contiguous()
-    if kind == 1:        # M[d+4][r*Cout+co][ci] = W[ci][co][-4d+r+13]
-        wp = torch.nn.functional.pad(w.reshape(c_in, c_out, KW), (3, 2))
+    if kind == 1:        # M[d+4][r*Cout+co][ci] = W[ci][co][-4d+r+deconv_padding(k)]
+        lp = _tap_pad(1, k)
+        wp = torch.nn.functional.pad(w.reshape(c_in, c_out, k), (lp, 36 - k - lp))
         return wp.view(c_in, c_out, 9, 4).flip(2).permute(2, 3, 1, 0).reshape(9, 4 * c_out, c_in).contiguous()
     return w.reshape(c_out, c_in, t_len).permute(0, 2, 1).reshape(1, c_out, t_len * c_in).contiguous()
 
 
-def unpack_reference(kind, m, c_out, c_in, t_len):
-    """Inverse of pack_reference (host-side twin of sg_unpack_wgrad without alpha)."""
+def unpack_reference(kind, m, c_out, c_in, t_len, k=31):
+    """Inverse of pack_reference (host-side twin of sg_unpack_wgrad_kw without alpha)."""
     if kind == 0:
-        return m.reshape(9, c_out, 4, c_in).permute(1, 3, 0, 2).reshape(c_out, c_in, 36)[..., 2:2 + KW].contiguous()
+        lp = _tap_pad(0, k)
+        return m.reshape(9, c_out, 4, c_in).permute(1, 3, 0, 2).reshape(c_out, c_in, 36)[..., lp:lp + k].contiguous()
     if kind == 1:
-        return m.reshape(9, 4, c_out, c_in).permute(3, 2, 0, 1).flip(2).reshape(c_in, c_out, 36)[..., 3:3 + KW].contiguous()
+        lp = _tap_pad(1, k)
+        return m.reshape(9, 4, c_out, c_in).permute(3, 2, 0, 1).flip(2).reshape(c_in, c_out, 36)[..., lp:lp + k].contiguous()
     return m.reshape(c_out, t_len, c_in).permute(0, 2, 1).reshape(c_out, c_in * t_len).contiguous()
 
 
@@ -694,10 +747,10 @@ class _NetEngine:
         if l.tied:
             src = torch.cat((src, src), 0).contiguous()          # both halves of the doubled input = the parameter
         if not dst.is_cuda:
-            dst.copy_(pack_reference(l.kind, src.float(), l.c_out, l.c_in, l.t_len).reshape(-1))
+            dst.copy_(pack_reference(l.kind, src.float(), l.c_out, l.c_in, l.t_len, l.kw).reshape(-1))
             return
-        _lib.call("sg_pack_weights", l.kind, _p(src), l.c_out, l.c_in, l.t_len, None, 0, _p(dst), None, SG_F32, SG_F32,
-                  _stream())
+        _lib.call("sg_pack_weights_kw", l.kind, _p(src), l.c_out, l.c_in, l.t_len, l.kw, None, 0, _p(dst), None, SG_F32,
+                  SG_F32, _stream())
 
     def _export(self, l, src, dst):
         """packed -> reference layout (pure layout transform)."""
@@ -710,9 +763,10 @@ class _NetEngine:
 
     def _export_plain(self, l, src, dst):
         if not src.is_cuda:
-            dst.copy_(unpack_reference(l.kind, src, l.c_out, l.c_in, l.t_len).reshape(dst.shape))
+            dst.copy_(unpack_reference(l.kind, src, l.c_out, l.c_in, l.t_len, l.kw).reshape(dst.shape))
             return
-        _lib.call("sg_unpack_wgrad", l.kind, _p(src), l.c_out, l.c_in, l.t_len, None, None, 0, _p(dst), None, 0, _stream())
+        _lib.call("sg_unpack_wgrad_kw", l.kind, _p(src), l.c_out, l.c_in, l.t_len, l.kw, None, None, 0, _p(dst), None, 0,
+                  _stream())
 
     def notice_external_writes(self):
         """Parameters written through torch since the last look (load_state_dict, init functions, p.data.copy_):
@@ -845,24 +899,24 @@ class _NetEngine:
 # --------------------------------------------------------------------------------------------
 def sn_v_layout(pl):
     """(reference shape of weight_v as a weight with one output channel, c_in of that weight) of packed layer `pl`.
-    Conv1d (dim 0): v runs over (ci, k) -> [1][Cin][31]; ConvTranspose1d (dim 1): v runs over (ci, k) of
-    W[Cin][Cout][31] -> [Cin][1][31]; a tied master holds [W | W], whose v covers one half."""
+    Conv1d (dim 0): v runs over (ci, k) -> [1][Cin][kw]; ConvTranspose1d (dim 1): v runs over (ci, k) of
+    W[Cin][Cout][kw] -> [Cin][1][kw]; a tied master holds [W | W], whose v covers one half."""
     vin = pl.c_in // 2 if pl.tied else pl.c_in
     if pl.kind == 0:
-        return (1, vin, KW), vin
+        return (1, vin, pl.kw), vin
     if pl.kind == 1:
-        return (vin, 1, KW), vin
+        return (vin, 1, pl.kw), vin
     return (1, -1), vin
 
 
 def sn_pack_v(pl, vref):
     """weight_v (reference layout, flat) -> the packed slots the power iteration of `pl` runs on."""
     shape, vin = sn_v_layout(pl)
-    return pack_reference(pl.kind, vref.reshape(shape), 1, vin, pl.t_len).reshape(-1).contiguous()
+    return pack_reference(pl.kind, vref.reshape(shape), 1, vin, pl.t_len, pl.kw).reshape(-1).contiguous()
 
 
 def sn_unpack_v(pl, v):
-    return unpack_reference(pl.kind, v, 1, sn_v_layout(pl)[1], pl.t_len).reshape(-1)
+    return unpack_reference(pl.kind, v, 1, sn_v_layout(pl)[1], pl.t_len, pl.kw).reshape(-1)
 
 
 def sn_geometry(pl):
@@ -955,6 +1009,9 @@ class GeneratorEngine(_SpectralNorm, _NetEngine):
         # .bias, small region of the bucket) and has no alpha -- every alpha use below reads 1
         self.conv_skip = self.has_skip and getattr(m, "skip_type", "alpha") == "conv"
         self.skip_kw = getattr(m, "skip_kwidth", 11)
+        # kernel width of every encoder conv and decoder deconv (31 in SEGAN+; Generator._served admits 4..32)
+        self.kw_enc = [b.kwidth for b in m.enc_blocks]
+        self.kw_dec = [b.kwidth for b in m.dec_blocks]
         self.packed = {}
         # norm_type='snorm' (modules.py:12-14): every encoder conv (dim 0) and decoder deconv (dim 1) is divided by its
         # spectral norm, re-estimated by one power iteration per training forward; the parameters are then called
@@ -963,6 +1020,11 @@ class GeneratorEngine(_SpectralNorm, _NetEngine):
         self.wsfx = "_orig" if self.snorm else ""
         self.sn = {}
         self._sn_reset()
+
+    def _require_wave_route(self):
+        if not wave_on_tensor_cores() and any(k != 31 for k in self.kw_enc + self.kw_dec):
+            raise NotImplementedError("Generator kernel widths other than 31 need the tensor-core waveform route "
+                                      "(SEGAN_B200_WAVE=tc)")
 
     def _sn_reset(self):
         # Pass slots: a forward that a backward will follow takes a slot that is neither outstanding (forward run,
@@ -992,8 +1054,8 @@ class GeneratorEngine(_SpectralNorm, _NetEngine):
                                   "Wt%d" % l, "Wtd%d" % l,
                                   alpha_name=(("alpha_%d.skip_k" % (nl - 1 - l))
                                               if l > 0 and self.has_skip and not self.conv_skip else None),
-                                  tied=(self.sum_merge and l > 0)))
-        ls += [PackedLayer(self.wname("enc", l), 0, fm[l], fm[l - 1], 0, "Wf%d" % l, "Wdg%d" % l)
+                                  tied=(self.sum_merge and l > 0), kw=self.kw_dec[l]))
+        ls += [PackedLayer(self.wname("enc", l), 0, fm[l], fm[l - 1], 0, "Wf%d" % l, "Wdg%d" % l, kw=self.kw_enc[l])
                for l in range(nl - 1, 0, -1)]
         return ls
 
@@ -1096,7 +1158,7 @@ class GeneratorEngine(_SpectralNorm, _NetEngine):
             w0 = w0 * self.sn_inv_sigma(self.wname("enc", 0))
         if self.sum_merge:                      # tied halves: W (hi + alpha skip) = [W | alpha W] cat(hi, skip)
             w = torch.cat((w, w), 0)
-        self.packed["w_last_dup"] = w.reshape(w.shape[0], 1, KW).contiguous()
+        self.packed["w_last_dup"] = w.reshape(w.shape[0], 1, self.kw_dec[l]).contiguous()
         weff = w.clone()
         if self.has_skip:
             half = w.shape[0] // 2
@@ -1105,11 +1167,11 @@ class GeneratorEngine(_SpectralNorm, _NetEngine):
         # tensor-core route of the waveform-end layers: single-tap operands (tiny tensors, torch ops)
         wcol = wave_col_weights(w0, dev)
         self.packed["Wcol0"] = wcol.half().contiguous()
-        kidx = dec_last_tap_index(dev)
+        kidx = dec_last_tap_index(dev, self.kw_dec[l])
         w2 = weff.t()[kidx.clamp(min=0)] * (kidx >= 0).float().unsqueeze(1)       # [64][cin]
         self.packed["W2_last"] = w2.half().contiguous()
         wg = torch.zeros(weff.shape[0], 64, dtype=torch.float32, device=dev)
-        wg[:, :KW] = weff
+        wg[:, :self.kw_dec[l]] = weff
         self.packed["Wg_last"] = wg.to(GT).contiguous()
         self._mark_packed("small")
         if self.conv_skip:
@@ -1193,6 +1255,7 @@ class GeneratorEngine(_SpectralNorm, _NetEngine):
         training (snorm only, the module's mode): one power iteration that updates weight_u / weight_v; eval mode
         uses the stored vectors and leaves them unchanged."""
         _require_cuda(x, z)
+        self._require_wave_route()
         twins = want_ctx if twins is None else (twins and want_ctx)
         bwd = twins                               # a backward pass will read this forward's saved tensors
         alias = twins and not grad_twins()        # fp16 gradients: the weight-gradient GEMMs read the forward tensors
@@ -1248,7 +1311,8 @@ class GeneratorEngine(_SpectralNorm, _NetEngine):
             if l == 0 and wave_on_tensor_cores():
                 col16 = buf.get("g.col16", (B, Lq[0], 64), F16, dev)
                 colb = buf.get("g.colb", (B, Lq[0], 64), GT, dev) if twins else None
-                _lib.call("sg_wave_im2col", _p(x), None, 1, B, L, 0, None, 1, 14, _p(col16), _p(colb), st)
+                _lib.call("sg_wave_im2col_kw", _p(x), None, 1, B, L, 0, None, 1, conv_offset(self.kw_enc[0]),
+                          self.kw_enc[0], _p(col16), _p(colb), st)
                 if alias:
                     colb = col16
                 self.wait_packed("small")
@@ -1262,8 +1326,10 @@ class GeneratorEngine(_SpectralNorm, _NetEngine):
             else:
                 cin = fm[l - 1]
                 self.wait_packed("Wf%d" % l)
+                taps = tap_ranges("conv_fwd", cin, 4 * cin, cout, self.kw_enc[l])
+                d_lo, d_hi = tap_span(taps)
                 run_f(hp[l - 1], None, Lq[l], 4, SG_F16, self.packed["Wf%d" % l], SG_F16, 4 * cin, cout,
-                      tap_ranges("conv_fwd", cin, 4 * cin, cout), a[l], SG_F16, Lq[l], 0, 0, Lq[l], B,
+                      taps, a[l], SG_F16, Lq[l], 0, 0, Lq[l], B, d_lo=d_lo, d_hi=d_hi,
                       bias=bias, bias_mod=cout, backend=self.backend, **fkw)
             if twins:
                 hpb[l] = buf.get("g.hpb%d" % l, (B, Lq[l] + 2 * halo, cout), GT, dev)
@@ -1310,8 +1376,10 @@ class GeneratorEngine(_SpectralNorm, _NetEngine):
                 fkw = dict(out2=dd[l], slope=slope, slope_mod=cout) if fz else {}
                 dst = ad[l]
             self.wait_packed("Wt%d" % l)
+            taps = tap_ranges("deconv_fwd", cout, cin, 4 * cout, self.kw_dec[l])
+            d_lo, d_hi = tap_span(taps)
             run_f(src0, src1, lin, 0, SG_F16, self.packed["Wt%d" % l], SG_F16, cin, 4 * cout,
-                  tap_ranges("deconv_fwd", cout, cin, 4 * cout), dst, SG_F16, lin, 0, 0, lin, B,
+                  taps, dst, SG_F16, lin, 0, 0, lin, B, d_lo=d_lo, d_hi=d_hi,
                   bias=self.pview("dec_blocks.%d.deconv.bias" % l), bias_mod=cout,
                   a0_c=src0.shape[-1], a1_c=c1, backend=self.backend, **fkw)
             if twins:
@@ -1456,8 +1524,9 @@ class GeneratorEngine(_SpectralNorm, _NetEngine):
         if wave_on_tensor_cores():
             _lib.call("sg_tanh_bwd", _p(gy), _p(ctx["y"]), B * L, _p(gpre), _p(gb), st)
             colg = buf.get("g.colg", (B, lin, 64), GT, dev)
-            _lib.call("sg_wave_im2col", _p(gpre), None, 1, B, L, 0, None, 0, 13, _p(colg) if GS == SG_F16 else None,
-                      _p(colg) if GS != SG_F16 else None, st)
+            kl = self.kw_dec[l]
+            _lib.call("sg_wave_im2col_kw", _p(gpre), None, 1, B, L, 0, None, 0, deconv_padding(kl), kl,
+                      _p(colg) if GS == SG_F16 else None, _p(colg) if GS != SG_F16 else None, st)
             if self.conv_skip:
                 for dst, n0 in ((g_in, 0), (buf.get("g.gsk0", (B, lin, half), GT, dev), half)):
                     run_f(colg, None, lin, 0, GS, self.packed["Wg_last"], GS, 64, cin, tap_ranges("full", 0, 64, cin),
@@ -1475,8 +1544,8 @@ class GeneratorEngine(_SpectralNorm, _NetEngine):
                     run_w(colg, lin // 2, GS, ctx["ddb"][l - 1], None, lin // 2, 0, GS, 2 * cin, 128,
                           tap_ranges("full", 0, 2 * cin, 128), dwq, B, d_lo=0, d_hi=0, dw_tap0=4, ksplit=74,
                           a0_c=2 * cin, backend=self.backend)
-                    _lib.call("sg_last_deconv_wgrad_fold_1src", _p(dwq), cin, _p(wgrad_dst(self.wname("dec", l))),
-                              _stream())
+                    _lib.call("sg_last_deconv_wgrad_fold_1src_kw", _p(dwq), cin, kl,
+                              _p(wgrad_dst(self.wname("dec", l))), _stream())
                     if sn_small:
                         self._sn_fix_small(self.wname("dec", l), sn_small[self.wname("dec", l)], slot)
             else:
@@ -1487,9 +1556,9 @@ class GeneratorEngine(_SpectralNorm, _NetEngine):
                           a0_c=cin, a1_c=cin, backend=self.backend)
                     gw_dst = wgrad_dst(self.wname("dec", l))
                     if self.sum_merge:
-                        gw_dst = buf.get("g.gw_last2", (cin, 1, KW), F32, dev, zero=True)
+                        gw_dst = buf.get("g.gw_last2", (cin, 1, kl), F32, dev, zero=True)
                     # snorm: w_last_dup is W / sigma, so the fold's dalpha is <dWeff, W~> as the reference's
-                    _lib.call("sg_last_deconv_wgrad_fold", _p(dwq), half, _p(self.packed["w_last_dup"]),
+                    _lib.call("sg_last_deconv_wgrad_fold_kw", _p(dwq), half, kl, _p(self.packed["w_last_dup"]),
                               _p(self.alpha_for_dec(l)), _p(gw_dst),
                               _p(self.gview("alpha_0.skip_k").view(-1)) if a_train else None, _stream())
                     if self.sum_merge:
@@ -1502,7 +1571,7 @@ class GeneratorEngine(_SpectralNorm, _NetEngine):
                                           "route (SEGAN_B200_WAVE=tc)")
             if self.conv_skip:
                 raise NotImplementedError("skip_type='conv' needs the tensor-core waveform route (SEGAN_B200_WAVE=tc)")
-            dweff = buf.get("g.dweff", (cin, KW), F32, dev, zero=True)
+            dweff = buf.get("g.dweff", (cin, self.kw_dec[l]), F32, dev, zero=True)
             _lib.call("sg_wave_deconv_bwd", _p(src0), half, _p(src1), half, B, lin, _p(self.packed["w_last_eff"]),
                       _p(gy), _p(ctx["y"]), _p(gpre), _p(g_in), _p(dweff), _p(gb), st)
             if self.sum_merge:
@@ -1532,12 +1601,14 @@ class GeneratorEngine(_SpectralNorm, _NetEngine):
             else:
                 s0, s1 = ctx["ddb"][l - 1], (ctx["skb"][nl - 1 - l] if self.has_skip else None)
             c0, c1 = s0.shape[-1], (0 if s1 is None else s1.shape[-1])
-            taps = tap_ranges("deconv_fwd", cout, cin, 4 * cout)
+            taps = tap_ranges("deconv_fwd", cout, cin, 4 * cout, self.kw_dec[l])
+            d_lo, d_hi = tap_span(taps)
+            taps_dg = tap_ranges("deconv_dgrad", cout, 4 * cout, cin, self.kw_dec[l])
             dwp = self.mgrad(self.by_name[self.wname("dec", l)])     # packed gradient slot (dWeff; snorm: / sigma)
             with on_side(side):
                 n_tiles = 9 * (4 * cout // 128) * max(1, cin // 256)
-                run_w(g_ad, lin, GS, s0, s1, lin, 0, GS, cin, 4 * cout, taps, dwp, B,
-                      ksplit=wgrad_ksplit(B * lin, n_tiles, taps, cin, 4 * cout), a0_c=c0, a1_c=c1,
+                run_w(g_ad, lin, GS, s0, s1, lin, 0, GS, cin, 4 * cout, taps, dwp, B, d_lo=d_lo, d_hi=d_hi,
+                      ksplit=wgrad_ksplit(B * lin, n_tiles, taps, cin, 4 * cout, d_lo, d_hi), a0_c=c0, a1_c=c1,
                       backend=self.backend, out_scale=osc(self.wname("dec", l)))
                 if l == 0 and reducer is not None:
                     reducer.ready(0, launch=True)              # every decoder weight gradient has been enqueued
@@ -1547,12 +1618,12 @@ class GeneratorEngine(_SpectralNorm, _NetEngine):
                 g_in = buf.get("g.gin%d" % l, (B, lin, cin // 2), GT, dev)
                 for dst, n0 in ((g_in, 0), (buf.get("g.gsk%d" % (nl - 1 - l), (B, lin, cin // 2), GT, dev), cin // 2)):
                     run_f(g_ad, None, lin, 0, GS, self.packed["Wtd%d" % l], GS, 4 * cout, cin,
-                          tap_ranges("deconv_dgrad", cout, 4 * cout, cin), dst, GS, lin, 0, 0, lin, B,
+                          taps_dg, dst, GS, lin, 0, 0, lin, B, d_lo=-d_hi, d_hi=-d_lo,
                           n_lo=n0, n_hi=n0 + cin // 2, out_ld=cin // 2, out_col0=0, backend=self.backend)
             else:
                 g_in = buf.get("g.gin%d" % l, (B, lin, cin), GT, dev)
                 run_f(g_ad, None, lin, 0, GS, self.packed["Wtd%d" % l], GS, 4 * cout, cin,
-                      tap_ranges("deconv_dgrad", cout, 4 * cout, cin), g_in, GS, lin, 0, 0, lin, B,
+                      taps_dg, g_in, GS, lin, 0, 0, lin, B, d_lo=-d_hi, d_hi=-d_lo,
                       n_lo=(self.zc if l == 0 else 0), n_hi=cin, backend=self.backend)
             g_next = g_in
         # ---- encoder blocks nl-1 .. 0
@@ -1586,7 +1657,8 @@ class GeneratorEngine(_SpectralNorm, _NetEngine):
                         run_w(g_a, Lq[0] // 2, GS, ctx["colb"], None, Lq[0] // 2, 0, GS, 128, 128,
                               tap_ranges("full", 0, 128, 128), dwq, B, d_lo=0, d_hi=0, dw_tap0=4, ksplit=148,
                               backend=self.backend)
-                        _lib.call("sg_wave_wgrad_fold", _p(dwq), 1, _p(wgrad_dst(self.wname("enc", 0))), _stream())
+                        _lib.call("sg_wave_wgrad_fold_kw", _p(dwq), 1, self.kw_enc[0],
+                                  _p(wgrad_dst(self.wname("enc", 0))), _stream())
                     else:
                         _lib.call("sg_wave_conv_wgrad", _p(ctx["x"]), None, 1, B, L, 0, _p(g_a), cout,
                                   _p(self.gview("enc_blocks.0.conv.weight")), None, _stream())
@@ -1596,19 +1668,20 @@ class GeneratorEngine(_SpectralNorm, _NetEngine):
             sn_coef(red, self.pview("enc_blocks.%d.conv.bias" % l) if self.enc_bias else None, cout,
                     self.wname("enc", l))
             cin = fm[l - 1]
-            taps = tap_ranges("conv_fwd", cin, 4 * cin, cout)
+            taps = tap_ranges("conv_fwd", cin, 4 * cin, cout, self.kw_enc[l])
+            d_lo, d_hi = tap_span(taps)
             dwp_l = self.mgrad(self.by_name[self.wname("enc", l)])
             with on_side(side):
                 n_tiles = 9 * (cout // 128) * max(1, 4 * cin // 256)
                 run_w(g_a, Lq[l], GS, ctx["hpb"][l - 1], None, Lq[l], 4, GS, 4 * cin, cout, taps, dwp_l, B,
-                      ksplit=wgrad_ksplit(B * Lq[l], n_tiles, taps, 4 * cin, cout), backend=self.backend,
-                      out_scale=osc(self.wname("enc", l)))
+                      d_lo=d_lo, d_hi=d_hi, ksplit=wgrad_ksplit(B * Lq[l], n_tiles, taps, 4 * cin, cout, d_lo, d_hi),
+                      backend=self.backend, out_scale=osc(self.wname("enc", l)))
                 if l == nl - 1 and reducer is not None:
                     reducer.ready(1, launch=True)
             g_hp = buf.get("g.ghp%d" % (l - 1), (B, Lq[l] + 8, 4 * cin), GT, dev)
             run_f(g_a, None, Lq[l], 0, GS, self.packed["Wdg%d" % l], GS, cout, 4 * cin,
-                  tap_ranges("conv_dgrad", cin, cout, 4 * cin), g_hp, GS, Lq[l], 4, -4, Lq[l] + 4, B,
-                  backend=self.backend)
+                  tap_ranges("conv_dgrad", cin, cout, 4 * cin, self.kw_enc[l]), g_hp, GS, Lq[l], 4, -4, Lq[l] + 4, B,
+                  d_lo=-d_hi, d_hi=-d_lo, backend=self.backend)
         join_side(side)
         if reducer is not None:
             reducer.ready(2, launch=True)
@@ -1651,6 +1724,7 @@ class DiscriminatorEngine(_SpectralNorm, _NetEngine):
         super().__init__(module)
         self.fmaps = list(module.fmaps)
         self.nl = len(self.fmaps)
+        self.kw = module.enc_blocks[0].kwidth          # one width for every tower conv (Discriminator._served: 4..32)
         self.packed = {}
         self.eps = 1e-5
         self.momentum = 0.1
@@ -1681,7 +1755,8 @@ class DiscriminatorEngine(_SpectralNorm, _NetEngine):
             ls.append(PackedLayer("fc.0.weight" + self.wsfx, 2, nout, fm[-1], kin // fm[-1], "W1p", "W1dg"))
         elif self.pool_type == "mlp":        # Conv1d(C, C, 1) weight [C][C][1] = a Linear with t_len 1
             ls.append(PackedLayer("mlp.0.weight" + self.wsfx, 2, fm[-1], fm[-1], 1, "Wm0", "Wm0dg"))
-        ls += [PackedLayer("enc_blocks.%d.conv.weight%s" % (l, self.wsfx), 0, fm[l], fm[l - 1], 0, "Wf%d" % l, "Wdg%d" % l)
+        ls += [PackedLayer("enc_blocks.%d.conv.weight%s" % (l, self.wsfx), 0, fm[l], fm[l - 1], 0, "Wf%d" % l, "Wdg%d" % l,
+                           kw=self.kw)
                for l in range(self.nl - 1, 0, -1)]
         return ls
 
@@ -1752,6 +1827,9 @@ class DiscriminatorEngine(_SpectralNorm, _NetEngine):
         device int32 tensor holding the same nl shifts; the kernels then read them from memory (no
         per-step scalar in the launches, so the step can be replayed from a CUDA graph)."""
         _require_cuda(x0, x1)
+        if self.kw != 31 and not wave_on_tensor_cores():
+            raise NotImplementedError("Discriminator kernel widths other than 31 need the tensor-core waveform route "
+                                      "(SEGAN_B200_WAVE=tc)")
         alias = twins and not grad_twins()
         twins = twins and grad_twins()
         sn_slot = None
@@ -1799,7 +1877,8 @@ class DiscriminatorEngine(_SpectralNorm, _NetEngine):
             if l == 0 and wave_on_tensor_cores():
                 col16 = buf.get("d.col16", (B, Lq[0], 64), F16, dev)
                 colb0 = buf.get("d.colb", (B, Lq[0], 64), GT, dev) if twins else None
-                _lib.call("sg_wave_im2col", _p(x0), _p(x1), 2, B, L, int(shifts[0]), rptr(0), 1, 14, _p(col16), _p(colb0), st)
+                _lib.call("sg_wave_im2col_kw", _p(x0), _p(x1), 2, B, L, int(shifts[0]), rptr(0), 1, conv_offset(self.kw),
+                          self.kw, _p(col16), _p(colb0), st)
                 if alias:
                     colb0 = col16
                 self.wait_packed("small")
@@ -1816,8 +1895,10 @@ class DiscriminatorEngine(_SpectralNorm, _NetEngine):
             else:
                 cin = fm[l - 1]
                 self.wait_packed("Wf%d" % l)
+                taps = tap_ranges("conv_fwd", cin, 4 * cin, cout, self.kw)
+                d_lo, d_hi = tap_span(taps)
                 run_f(hp[l - 1], None, Lq[l], 4, SG_F16, self.packed["Wf%d" % l], SG_F16, 4 * cin, cout,
-                      tap_ranges("conv_fwd", cin, 4 * cin, cout), a[l], SG_F16, Lq[l], 0, 0, Lq[l], B,
+                      taps, a[l], SG_F16, Lq[l], 0, 0, Lq[l], B, d_lo=d_lo, d_hi=d_hi,
                       bias=bias, bias_mod=cout, backend=self.backend, stats=stats[l] if fuse_stats else None)
             bn = m.enc_blocks[l].norm
             if bnorm:
@@ -2089,7 +2170,7 @@ class DiscriminatorEngine(_SpectralNorm, _NetEngine):
                         run_w(g_a, Lq[0] // 2, GS, ctx["colb"], None, Lq[0] // 2, 0, GS, 128, 128,
                               tap_ranges("full", 0, 128, 128), dwq, B, d_lo=0, d_hi=0, dw_tap0=4, ksplit=148,
                               backend=self.backend)
-                        _lib.call("sg_wave_wgrad_fold", _p(dwq), 2, _p(g_w0), _stream())
+                        _lib.call("sg_wave_wgrad_fold_kw", _p(dwq), 2, self.kw, _p(g_w0), _stream())
                         if sn_small:
                             self._sn_fix_small("enc_blocks.0.conv.weight_orig",
                                                sn_small["enc_blocks.0.conv.weight_orig"], slot)
@@ -2106,14 +2187,16 @@ class DiscriminatorEngine(_SpectralNorm, _NetEngine):
                           tap_ranges("full", 0, 64, 64), P2, GS, Lq[0], 0, 0, Lq[0], B, d_lo=0, d_hi=0, w_tap0=4,
                           backend=self.backend)
                     if input_grad is not None:
-                        _lib.call("sg_wave_col2im_fold", _p(P2), 0, B, L, shifts[0], rptr(0), _p(input_grad), st)
+                        _lib.call("sg_wave_col2im_fold_kw", _p(P2), 0, B, L, shifts[0], rptr(0), self.kw,
+                                  _p(input_grad), st)
                     if input_grad1 is not None:
-                        _lib.call("sg_wave_col2im_fold", _p(P2), 32, B, L, shifts[0], rptr(0), _p(input_grad1), st)
+                        _lib.call("sg_wave_col2im_fold_kw", _p(P2), 32, B, L, shifts[0], rptr(0), self.kw,
+                                  _p(input_grad1), st)
                 else:
                     if input_grad is not None:
                         _lib.call("sg_wave_conv_dgrad", _p(g_a), B, L, shifts[0], _p(w0), 2, cout, _p(input_grad), 1, st)
                     if input_grad1 is not None:     # gradient w.r.t. the second input channel
-                        w1 = C.c_void_p(w0.data_ptr() + 4 * KW)
+                        w1 = C.c_void_p(w0.data_ptr() + 4 * self.kw)
                         _lib.call("sg_wave_conv_dgrad", _p(g_a), B, L, shifts[0], w1, 2, cout, _p(input_grad1), 1, st)
                 break
             cin = fm[l - 1]
@@ -2123,18 +2206,20 @@ class DiscriminatorEngine(_SpectralNorm, _NetEngine):
                 osc = self.sn_inv_sigma(pl_l.name, slot) if sn else None
                 with on_side(side):
                     n_tiles = 9 * (cout // 128) * max(1, 4 * cin // 256)
-                    taps_w = tap_ranges("conv_fwd", cin, 4 * cin, cout)
+                    taps_w = tap_ranges("conv_fwd", cin, 4 * cin, cout, self.kw)
+                    d_lo, d_hi = tap_span(taps_w)
                     run_w(g_a, Lq[l], GS, ctx["hpb"][l - 1], None, Lq[l], 4, GS, 4 * cin, cout, taps_w, dwp_l, B,
-                          ksplit=wgrad_ksplit(B * Lq[l], n_tiles, taps_w, 4 * cin, cout), backend=self.backend,
-                          out_scale=osc)
+                          d_lo=d_lo, d_hi=d_hi, ksplit=wgrad_ksplit(B * Lq[l], n_tiles, taps_w, 4 * cin, cout, d_lo,
+                                                                    d_hi), backend=self.backend, out_scale=osc)
                     if l == nl - 1 and reducer is not None:
                         # fc.0 and enc4 of THIS pass are enqueued; the chunk leaves once every accumulating pass
                         # (real / fake / misaligned ...) has said so: reduce_now marks the last one
                         reducer.ready(0, launch=reduce_now)
             g_h = buf.get("d.gh%d" % (l - 1), (B, Lq[l] + 8, 4 * cin), GT, dev)
+            taps_dg = tap_ranges("conv_dgrad", cin, cout, 4 * cin, self.kw)
+            d_lo, d_hi = tap_span(taps_dg)
             run_f(g_a, None, Lq[l], 0, GS, self.packed["Wdg%d" % l], GS, cout, 4 * cin,
-                  tap_ranges("conv_dgrad", cin, cout, 4 * cin), g_h, GS, Lq[l], 4, -4, Lq[l] + 4, B,
-                  backend=self.backend)
+                  taps_dg, g_h, GS, Lq[l], 4, -4, Lq[l] + 4, B, d_lo=d_lo, d_hi=d_hi, backend=self.backend)
         join_side(side)
         if reducer is not None and param_grads:
             reducer.ready(1, launch=reduce_now)

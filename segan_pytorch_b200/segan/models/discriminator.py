@@ -123,15 +123,20 @@ class Discriminator(Model):
         self.fmaps = list(fmaps)
         self.bias = bias
         self.norm_type = norm_type
-        self._served = (ninputs == 2 and norm_type in ('bnorm', 'snorm') and bias and kwidth == 31 and all(p == 4 for p in poolings)
+        self._served = (ninputs == 2 and norm_type in ('bnorm', 'snorm') and bias and _engine.kwidth_served(kwidth)
+                        and all(p == 4 for p in poolings)
                         and fmaps[0] == 64 and all(f % 64 == 0 for f in fmaps) and len(fmaps) >= 2)
+        self._unserved = ("this Discriminator configuration is outside the built hot path "
+                          "(SEGAN+ defaults: 2 input channels, bnorm or snorm, kernel width 4-32, stride 4)")
+        if not _engine.kwidth_served(kwidth):
+            self._unserved = ("kernel width kwidth=%r is not served: it must be an integer in 4-32 (the first layer's "
+                              "im2col holds 32 taps per input channel)" % (kwidth,))
         self._engine = None
 
     @property
     def engine(self):
         if not self._served:
-            raise NotImplementedError("this Discriminator configuration is outside the built hot path "
-                                      "(SEGAN+ defaults: 2 input channels, bnorm or snorm, k=31, stride 4)")
+            raise NotImplementedError(self._unserved)
         if self._engine is None:
             self._engine = _engine.DiscriminatorEngine(self)
         return self._engine

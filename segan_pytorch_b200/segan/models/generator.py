@@ -2,8 +2,9 @@
 
 Same constructor signature, same `forward(x, z=None, ret_hid=False)` contract, same state-dict
 keys; the arithmetic runs in libsegan_b200.so (segan_pytorch_b200.engine.GeneratorEngine).  Served: alpha / constant /
-conv skips with concat or sum merge, skip=False, no_z=True, any z_dim that is a positive multiple of 64, and
-norm_type None or 'snorm' (spectrally normalised encoder convs and decoder deconvs)."""
+conv skips with concat or sum merge, skip=False, no_z=True, any z_dim that is a positive multiple of 64,
+norm_type None or 'snorm' (spectrally normalised encoder convs and decoder deconvs), and every kernel width
+4 <= k <= 32 for each encoder conv (kwidth) and decoder deconv (dec_kwidth)."""
 import torch
 import torch.nn as nn
 
@@ -144,14 +145,18 @@ class Generator(Model):
                                                             or (skip_type == 'conv'
                                                                 and _engine.skipconv_served(skip_kwidth)))))
                         and norm_type in (None, 'snorm')
-                        and all(k == 31 for k in kwidth) and all(k == 31 for k in dec_kwidth)
+                        and all(_engine.kwidth_served(k) for k in list(kwidth) + list(dec_kwidth))
                         and all(p == 4 for p in poolings) and all(p == 4 for p in dec_poolings)
                         and list(dec_fmaps) == fmaps[::-1][1:] + [1]
                         and all(f % 64 == 0 for f in fmaps) and fmaps[0] == 64)
         self.norm_type = norm_type
         self._unserved = None if self._served else ("this Generator configuration is outside the built hot path "
-                                                     "(SEGAN+ layout: k=31, stride 4, norm_type None or 'snorm', "
-                                                     "fmaps 64..)")
+                                                     "(SEGAN+ layout: kernel widths 4-32, stride 4, norm_type None "
+                                                     "or 'snorm', fmaps 64..)")
+        if not all(_engine.kwidth_served(k) for k in list(kwidth) + list(dec_kwidth)):
+            self._unserved = ("kernel widths kwidth=%r / dec_kwidth=%r are not served: every width must be an integer "
+                              "in 4-32 (the waveform-end im2col holds 32 taps per channel; below 4 the transposed "
+                              "conv does not give 4x its input length)" % (list(kwidth), list(dec_kwidth)))
         if norm_type == 'bnorm':
             self._unserved = ("norm_type='bnorm' is not served for the Generator: the Generator's kernels have no "
                               "BatchNorm between a convolution and its PReLU (norm_type None and 'snorm' are served)")
