@@ -201,6 +201,13 @@ def tap_span(taps):
     return live[0], live[-1]
 
 
+def dgrad_span(fwd_taps):
+    """(d_lo, d_hi) of a layer's data-gradient tap-GEMM from its forward tap table: data-gradient tap d is the
+    transpose of forward tap -d, so the span is the forward span mirrored (= tap_span of the data-gradient table)."""
+    d_lo, d_hi = tap_span(fwd_taps)
+    return -d_hi, -d_lo
+
+
 # optional live profiling (bench.py): list of (kind, start_event, end_event, algorithmic_flops)
 PROFILE = None
 
@@ -1604,6 +1611,7 @@ class GeneratorEngine(_SpectralNorm, _NetEngine):
             taps = tap_ranges("deconv_fwd", cout, cin, 4 * cout, self.kw_dec[l])
             d_lo, d_hi = tap_span(taps)
             taps_dg = tap_ranges("deconv_dgrad", cout, 4 * cout, cin, self.kw_dec[l])
+            dg_lo, dg_hi = dgrad_span(taps)
             dwp = self.mgrad(self.by_name[self.wname("dec", l)])     # packed gradient slot (dWeff; snorm: / sigma)
             with on_side(side):
                 n_tiles = 9 * (4 * cout // 128) * max(1, cin // 256)
@@ -1618,12 +1626,12 @@ class GeneratorEngine(_SpectralNorm, _NetEngine):
                 g_in = buf.get("g.gin%d" % l, (B, lin, cin // 2), GT, dev)
                 for dst, n0 in ((g_in, 0), (buf.get("g.gsk%d" % (nl - 1 - l), (B, lin, cin // 2), GT, dev), cin // 2)):
                     run_f(g_ad, None, lin, 0, GS, self.packed["Wtd%d" % l], GS, 4 * cout, cin,
-                          taps_dg, dst, GS, lin, 0, 0, lin, B, d_lo=-d_hi, d_hi=-d_lo,
+                          taps_dg, dst, GS, lin, 0, 0, lin, B, d_lo=dg_lo, d_hi=dg_hi,
                           n_lo=n0, n_hi=n0 + cin // 2, out_ld=cin // 2, out_col0=0, backend=self.backend)
             else:
                 g_in = buf.get("g.gin%d" % l, (B, lin, cin), GT, dev)
                 run_f(g_ad, None, lin, 0, GS, self.packed["Wtd%d" % l], GS, 4 * cout, cin,
-                      taps_dg, g_in, GS, lin, 0, 0, lin, B, d_lo=-d_hi, d_hi=-d_lo,
+                      taps_dg, g_in, GS, lin, 0, 0, lin, B, d_lo=dg_lo, d_hi=dg_hi,
                       n_lo=(self.zc if l == 0 else 0), n_hi=cin, backend=self.backend)
             g_next = g_in
         # ---- encoder blocks nl-1 .. 0
@@ -1679,9 +1687,10 @@ class GeneratorEngine(_SpectralNorm, _NetEngine):
                 if l == nl - 1 and reducer is not None:
                     reducer.ready(1, launch=True)
             g_hp = buf.get("g.ghp%d" % (l - 1), (B, Lq[l] + 8, 4 * cin), GT, dev)
+            dg_lo, dg_hi = dgrad_span(taps)
             run_f(g_a, None, Lq[l], 0, GS, self.packed["Wdg%d" % l], GS, cout, 4 * cin,
                   tap_ranges("conv_dgrad", cin, cout, 4 * cin, self.kw_enc[l]), g_hp, GS, Lq[l], 4, -4, Lq[l] + 4, B,
-                  d_lo=-d_hi, d_hi=-d_lo, backend=self.backend)
+                  d_lo=dg_lo, d_hi=dg_hi, backend=self.backend)
         join_side(side)
         if reducer is not None:
             reducer.ready(2, launch=True)

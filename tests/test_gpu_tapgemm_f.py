@@ -98,7 +98,7 @@ def _taps(c):
         return [list(t) for t in c["table"]], c["d"][0], c["d"][1], c.get("tap0", 0)
     ch = {"conv_fwd": kc // 4, "deconv_dgrad": kc // 4, "conv_dgrad": nc // 4, "deconv_fwd": nc // 4, "full": 0}[kind]
     d = c.get("d", (-4, 4))
-    return E.tap_ranges(kind, ch, kc, nc), d[0], d[1], c.get("tap0", 0)
+    return E.tap_ranges(kind, ch, kc, nc, c.get("k", 31)), d[0], d[1], c.get("tap0", 0)
 
 
 def _geom(c):
